@@ -65,6 +65,8 @@ typedef struct mgb200_graph_info {
   double build_ms;         /* device time of the CSR/SELL build                       */
   double upload_ms;        /* host COO -> device, wall clock (0 for create_device)    */
   uint64_t build_peak_bytes; /* device memory in use at the build's high-water mark   */
+  uint64_t tiled_edges;    /* heavy-row edges gathered from shared-memory tiles       */
+  uint64_t tile_chunks;    /* their (row, tile) runs of <= MGB200_TILE_CHUNK edges    */
 } mgb200_graph_info;
 
 typedef struct mgb200_run_stats {

@@ -612,6 +612,8 @@ int mgb200_graph_get_info(const mgb200_graph *h, mgb200_graph_info *info) {
   info->build_ms = g.build_ms;
   info->upload_ms = g.upload_ms;
   info->build_peak_bytes = g.build_peak_bytes;
+  info->tiled_edges = g.tiled_edges;
+  info->tile_chunks = g.tile_chunks;
   return MGB200_OK;
 }
 

@@ -25,6 +25,7 @@ namespace mgb200 {
 
 constexpr int kMaxPeers = 8;
 constexpr int kSliceRows = 32;
+constexpr uint32_t kMaxTileLabels = 28672;  // (T + 1) doubles of shared memory per tile; offsets (pad = T) fit 16 bits
 // When Graph::idx_flagged, a stored source index (heavy_idx / sell_idx) carries the hotness of its label:
 constexpr uint32_t kIdxL2Hot = 0x80000000u;     // keep in L2 (evict_last), else evict_first
 constexpr uint32_t kIdxL1Hot = 0x40000000u;     // may allocate in L1, else bypass
@@ -164,15 +165,37 @@ struct Graph {
   uint32_t *need_mask = nullptr;    // [ceil(local_rows / 4)] one BYTE per owned row: bit q = partition q gathers this
                                     // row's contribution (has an in-edge from it); nullptr = push to every peer
 
-  // heavy class
-  uint64_t heavy_edges = 0;
-  uint64_t *heavy_ptr = nullptr;  // [n_heavy + 1]
-  uint32_t *heavy_idx = nullptr;  // [heavy_edges] source labels (+ hot flags if idx_flagged), ascending inside a row
-  uint64_t n_seg = 0;
-  uint32_t *seg_row = nullptr;    // [n_seg] local heavy row
-  uint64_t *seg_begin = nullptr;  // [n_seg] first edge
-  uint64_t *seg_first = nullptr;  // [n_heavy + 1] first segment of each heavy row
+  // heavy class.  A heavy row's in-edges are split at the tile boundary (graph_build.cu TileSet): sources in the tiled
+  // hot prefix are summed from shared-memory tiles of contrib (tile chunks), the rest (cold edges) by edge segments.
+  // Row r owns partials [seg_first[r], seg_first[r + 1]): its tile chunks in tile order, then its cold segments.
+  uint64_t heavy_edges = 0;       // all in-edges of the heavy rows (tiled + cold)
+  uint64_t *heavy_ptr = nullptr;  // [n_heavy + 1] over the cold edges
+  uint32_t *heavy_idx = nullptr;  // [cold edges] source labels (+ hot flags if idx_flagged), ascending inside a row
+  uint64_t n_seg = 0;             // partials: tile chunks + cold segments
+  uint64_t n_cold_seg = 0;        // cold segments (heavy_segments_kernel)
+  uint32_t *seg_row = nullptr;    // [n_cold_seg] local heavy row
+  uint64_t *seg_begin = nullptr;  // [n_cold_seg] first cold edge
+  uint64_t *seg_slot = nullptr;   // [n_cold_seg] partial of each cold segment; nullptr = identity (no tile chunks)
+  uint64_t *seg_first = nullptr;  // [n_heavy + 1] first partial of each heavy row
   double *seg_partial = nullptr;  // [n_seg]
+
+  // tile class (unweighted graphs; MGB200_TILE_LABELS = 0 turns it off).  Tile t is contrib[tile_base[t] ..
+  // + tile_load[t]) (16-byte aligned, so one TMA bulk copy fills it); a tile chunk is <= tile_chunk consecutive edges
+  // of one heavy row whose sources lie in one tile.  Inside a tile the chunks are sorted by length and stored as
+  // SELL-32 slices of 16-bit tile offsets (column-major, one lane per chunk, padding = offset tile_labels -> 0.0).
+  uint64_t tiled_edges = 0, tile_chunks = 0;
+  uint32_t n_tiles = 0;
+  uint64_t tile_slices = 0;
+  uint32_t *tile_base = nullptr;        // [n_tiles]
+  uint32_t *tile_load = nullptr;        // [n_tiles] labels copied (even)
+  uint64_t *tile_slice_first = nullptr; // [n_tiles + 1] slices are tile-major
+  uint32_t *tslice_tile = nullptr;      // [tile_slices]
+  uint64_t *tslice_colbase = nullptr;   // [tile_slices + 1] in units of 32-entry columns
+  uint16_t *tile_idx = nullptr;         // [32 * columns] offset of the source inside its tile
+  uint64_t *tile_slot = nullptr;        // [32 * tile_slices] partial written by each lane; ~0 = padding lane
+  uint32_t tile_work = 0;               // work items = CTAs of heavy_tiles_kernel: contiguous slice runs, ~equal cost
+  uint64_t *tile_work_begin = nullptr;  // [tile_work + 1]
+  int tile_attr_bytes = 0;              // dynamic shared memory already granted to heavy_tiles_kernel
   double *heavy_sums = nullptr;   // [n_heavy] per-row gathered sums of the current iteration
   // optional edge weights (cuGraph-semantics variants only; one partition): parallel to heavy_idx / sell_idx, pad = 0
   double *heavy_w = nullptr, *sell_w = nullptr;
@@ -216,6 +239,10 @@ struct Graph {
   cudaStream_t stream2 = nullptr;
   cudaEvent_t fork_ev = nullptr;
   cudaEvent_t join_ev = nullptr;
+  // stream of the cold heavy segments, which run next to heavy_tiles_kernel (launch_heavy_gathers)
+  cudaStream_t cold_stream = nullptr;
+  cudaEvent_t cold_fork_ev = nullptr;
+  cudaEvent_t cold_join_ev = nullptr;
   bool overlap_epilogue = true;
   bool stream_attr_set = false;
   static constexpr int kOccSlots = 24;  // occupancy of every kernel launched on this handle, asked once (grid_for)
@@ -238,6 +265,9 @@ struct Graph {
     bool lone_partition = false; // MGB200_LONE_PARTITION=1 (profiling only): run ONE partition of part_world without its
                                  // peers -- no stores to them, barrier of one; timings are real, ranks are NOT
     int idx_flags = -1;          // MGB200_IDX_FLAGS: 1 bake hotness into the indices, 0 never, -1 (default) see build_graph
+    uint32_t tile_labels = 16384;  // MGB200_TILE_LABELS: labels per shared-memory tile (even, <= kMaxTileLabels; 0 = off)
+    uint64_t tile_hot_mb = 16;     // MGB200_TILE_HOT_MB: tiled prefix of contrib (split between the owners like L2_HOT_MB)
+    uint32_t tile_chunk = 256;     // MGB200_TILE_CHUNK: most edges of one tile chunk
     unsigned long long barrier_timeout_ms = 20000;  // MGB200_BARRIER_TIMEOUT_MS
   } tun;
   // hot thresholds in LOCAL label units (label - first label of the owning partition); one definition for the

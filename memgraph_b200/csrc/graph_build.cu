@@ -214,22 +214,158 @@ __global__ void low32_kernel(uint64_t count, const uint64_t *key, IndexFlags fla
     out[e] = flags(static_cast<uint32_t>(key[e]));
 }
 
-struct SegCount {
-  uint32_t seg;
-  __host__ __device__ uint64_t operator()(uint32_t deg) const { return (static_cast<uint64_t>(deg) + seg - 1) / seg; }
+// Which sources a heavy row gathers from shared-memory tiles: every owner's first `hot` labels (local label below
+// `hot`, like the L2 window's hot_divisor()) -- P owners under the dealt labelling, else one owner whose range is [0, n).
+// It depends on the labelling and the MGB200_TILE_* knobs only, never on the cache-policy knobs.
+struct TileSet {
+  Dealer owners;
+  uint64_t hot;
+  __device__ bool hot_label(uint32_t label) const {
+    uint64_t s0 = 0;
+    for (uint32_t q = 1; q < owners.world; ++q)
+      if (label >= owners.start(q)) s0 = owners.start(q);
+    return label - s0 < hot;
+  }
+};
+struct ColdKey {  // cub::DeviceSelect predicate: the edge's source is not tiled
+  TileSet ts;
+  __device__ bool operator()(uint64_t key) const { return !ts.hot_label(static_cast<uint32_t>(key)); }
 };
 
-__global__ void segment_fill_kernel(uint64_t n_heavy, const uint64_t *heavy_ptr, const uint64_t *seg_first,
-                                    uint32_t seg_edges, uint32_t *seg_row, uint64_t *seg_begin) {
-  // one warp per heavy row; lanes stride over that row's segments
+__device__ __forceinline__ uint64_t lower_bound_key(const uint64_t *key, uint64_t lo, uint64_t hi, uint64_t v) {
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if (key[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// (heavy row r, tile t) pairs, p = r * n_tiles + t: edges of r whose source lies in [tile_lo[t], tile_hi[t]) -- one
+// contiguous run of the row's ascending sources -- and the chunks of at most `chunk` edges they make
+__global__ void tile_pair_kernel(uint64_t n_heavy, uint32_t n_tiles, const uint64_t *row_ptr, const uint64_t *key,
+                                 const uint32_t *tile_lo, const uint32_t *tile_hi, uint32_t chunk, uint32_t *pair_cnt,
+                                 uint64_t *pair_chunks, unsigned long long *tile_chunks) {
+  const uint64_t pairs = n_heavy * n_tiles;
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t p = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; p < pairs; p += stride) {
+    const uint64_t r = p / n_tiles;
+    const uint32_t t = static_cast<uint32_t>(p % n_tiles);
+    const uint64_t e1 = row_ptr[r + 1];
+    const uint64_t lo = lower_bound_key(key, row_ptr[r], e1, (r << 32) | tile_lo[t]);
+    const uint64_t cnt = lower_bound_key(key, lo, e1, (r << 32) | tile_hi[t]) - lo;
+    const uint64_t nch = (cnt + chunk - 1) / chunk;
+    pair_cnt[p] = static_cast<uint32_t>(cnt);
+    pair_chunks[p] = nch;
+    if (nch) atomicAdd(tile_chunks + t, static_cast<unsigned long long>(nch));
+  }
+}
+
+// per heavy row: cold in-degree and tile chunks (no tiles: the in-degree and 0)
+__global__ void tile_row_kernel(uint64_t n_heavy, uint32_t n_tiles, const uint32_t *indeg_local, const uint32_t *pair_cnt,
+                                const uint64_t *pair_chunks, uint64_t *cold_deg, uint64_t *row_chunks) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n_heavy; r += stride) {
+    uint64_t hot = 0, chunks = 0;
+    for (uint32_t t = 0; t < n_tiles; ++t) {
+      hot += pair_cnt[r * n_tiles + t];
+      chunks += pair_chunks[r * n_tiles + t];
+    }
+    cold_deg[r] = indeg_local[r] - hot;
+    row_chunks[r] = chunks;
+  }
+}
+
+// per heavy row: partials (tile chunks + cold segments) and cold segments
+__global__ void seg_count_kernel(uint64_t n_heavy, const uint64_t *cold_deg, const uint64_t *row_chunks,
+                                 uint32_t seg_edges, uint64_t *row_parts, uint64_t *row_cold_segs) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n_heavy; r += stride) {
+    const uint64_t segs = (cold_deg[r] + seg_edges - 1) / seg_edges;
+    row_parts[r] = row_chunks[r] + segs;
+    row_cold_segs[r] = segs;
+  }
+}
+
+// one record per tile chunk, in row order (= partial order): sort key (tile, length descending), first edge, partial
+__global__ void tile_chunk_kernel(uint64_t n_heavy, uint32_t n_tiles, const uint64_t *row_ptr, const uint64_t *key,
+                                  const uint32_t *tile_lo, const uint32_t *pair_cnt, const uint64_t *pair_chunk_first,
+                                  const uint64_t *seg_first, uint32_t chunk, uint64_t *chunk_key, uint64_t *chunk_id,
+                                  uint64_t *chunk_begin, uint32_t *chunk_len, uint64_t *chunk_slot) {
+  const uint64_t pairs = n_heavy * n_tiles;
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t p = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; p < pairs; p += stride) {
+    const uint32_t cnt = pair_cnt[p];
+    if (cnt == 0) continue;
+    const uint64_t r = p / n_tiles;
+    const uint32_t t = static_cast<uint32_t>(p % n_tiles);
+    const uint64_t lo = lower_bound_key(key, row_ptr[r], row_ptr[r + 1], (r << 32) | tile_lo[t]);
+    const uint64_t c0 = pair_chunk_first[p], row_c0 = pair_chunk_first[r * n_tiles];
+    for (uint32_t k = 0; k * static_cast<uint64_t>(chunk) < cnt; ++k) {
+      const uint64_t c = c0 + k;
+      const uint32_t len = static_cast<uint32_t>(min(static_cast<uint64_t>(chunk), cnt - static_cast<uint64_t>(k) * chunk));
+      chunk_key[c] = (static_cast<uint64_t>(t) << 32) | (0xFFFFFFFFu - len);
+      chunk_id[c] = c;
+      chunk_begin[c] = lo + static_cast<uint64_t>(k) * chunk;
+      chunk_len[c] = len;
+      chunk_slot[c] = seg_first[r] + (c - row_c0);
+    }
+  }
+}
+
+// width of every tile slice = length of its first (longest) chunk
+__global__ void tile_width_kernel(uint64_t n_slices, const uint32_t *slice_tile, const uint64_t *tile_slice_first,
+                                  const uint64_t *tile_chunk_first, const uint64_t *sorted_id, const uint32_t *chunk_len,
+                                  uint64_t *width) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t s = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; s < n_slices; s += stride) {
+    const uint32_t t = slice_tile[s];
+    width[s] = chunk_len[sorted_id[tile_chunk_first[t] + (s - tile_slice_first[t]) * kSliceRows]];
+  }
+}
+
+// one warp per tile slice, lane l = chunk l of the slice: its offsets column-major, padded with `pad` (slot T = 0.0)
+__global__ void tile_fill_kernel(uint64_t n_slices, const uint32_t *slice_tile, const uint64_t *tile_slice_first,
+                                 const uint64_t *tile_chunk_first, const uint32_t *tile_base, const uint64_t *colbase,
+                                 const uint64_t *sorted_id, const uint64_t *chunk_begin, const uint32_t *chunk_len,
+                                 const uint64_t *chunk_slot, const uint64_t *key, uint16_t pad, uint16_t *tile_idx,
+                                 uint64_t *tile_slot) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t warps_total = static_cast<uint64_t>(gridDim.x) * (blockDim.x >> 5);
+  for (uint64_t s = static_cast<uint64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); s < n_slices;
+       s += warps_total) {
+    const uint32_t t = slice_tile[s];
+    const uint64_t p = tile_chunk_first[t] + (s - tile_slice_first[t]) * kSliceRows + lane;
+    const bool valid = p < tile_chunk_first[t + 1];
+    uint64_t begin = 0, slot = ~0ull;
+    uint32_t len = 0;
+    if (valid) {
+      const uint64_t c = sorted_id[p];
+      begin = chunk_begin[c];
+      len = chunk_len[c];
+      slot = chunk_slot[c];
+    }
+    const uint64_t c0 = colbase[s];
+    const uint32_t width = static_cast<uint32_t>(colbase[s + 1] - c0);
+    const uint32_t base = tile_base[t];
+    uint16_t *dst = tile_idx + c0 * kSliceRows + lane;
+    for (uint32_t k = 0; k < width; ++k)
+      dst[static_cast<size_t>(k) * kSliceRows] = k < len ? static_cast<uint16_t>(static_cast<uint32_t>(key[begin + k]) - base) : pad;
+    tile_slot[s * kSliceRows + lane] = slot;
+  }
+}
+
+__global__ void segment_fill_kernel(uint64_t n_heavy, const uint64_t *heavy_ptr, const uint64_t *cold_seg_first,
+                                    uint32_t seg_edges, const uint64_t *seg_first, uint32_t *seg_row, uint64_t *seg_begin, uint64_t *seg_slot) {
+  // one warp per heavy row; lanes stride over that row's cold segments, which follow its tile chunks in partial order
   const int lane = threadIdx.x & 31;
   const uint64_t warps_total = static_cast<uint64_t>(gridDim.x) * (blockDim.x >> 5);
   for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n_heavy;
        r += warps_total) {
-    const uint64_t s0 = seg_first[r], s1 = seg_first[r + 1], e0 = heavy_ptr[r];
+    const uint64_t s0 = cold_seg_first[r], s1 = cold_seg_first[r + 1], e0 = heavy_ptr[r];
     for (uint64_t s = s0 + lane; s < s1; s += 32) {
       seg_row[s] = static_cast<uint32_t>(r);
       seg_begin[s] = e0 + (s - s0) * seg_edges;
+      if (seg_slot) seg_slot[s] = seg_first[r + 1] - (s1 - s);  // the row's partials end with its cold segments
     }
   }
 }
@@ -341,6 +477,18 @@ struct Scratch {
   }
 };
 
+// out[0] = 0, out[i + 1] = in[0] + .. + in[i]: an exclusive scan that ends with the total
+template <typename It>
+cudaError_t prefix_sum(Scratch &tmp, It in, uint64_t *out, uint64_t count, cudaStream_t st) {
+  cudaError_t e = cudaMemsetAsync(out, 0, sizeof(uint64_t), st);
+  if (e != cudaSuccess || count == 0) return e;
+  size_t bytes = 0;
+  if ((e = cub::DeviceScan::InclusiveSum(nullptr, bytes, in, out + 1, count, st)) != cudaSuccess) return e;
+  void *cub_tmp = nullptr;
+  if ((e = tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes)) != cudaSuccess) return e;
+  return cub::DeviceScan::InclusiveSum(cub_tmp, bytes, in, out + 1, count, st);
+}
+
 template <typename T>
 cudaError_t keep_alloc(Graph &g, T **out, uint64_t count) {
   void *p = nullptr;
@@ -402,6 +550,10 @@ void free_graph(Graph &g) {
   if (g.heavy_w) cudaFree(g.heavy_w);
   if (g.sell_w) cudaFree(g.sell_w);
   if (g.outw_l) cudaFree(g.outw_l);
+  void *tile_ptrs[] = {g.seg_slot,  g.tile_base, g.tile_load, g.tile_slice_first, g.tslice_tile,
+                       g.tslice_colbase, g.tile_idx, g.tile_slot, g.tile_work_begin};
+  for (void *p : tile_ptrs)
+    if (p) cudaFree(p);
   void *ptrs[] = {g.label_of,  g.outdeg_l,  g.local_vertex, g.heavy_ptr,    g.heavy_idx, g.seg_row,     g.seg_begin,
                   g.seg_first, g.seg_partial, g.heavy_sums, g.sell_colbase, g.sell_idx,     g.rank,      g.window,      g.state,
                   g.sum_partials};
@@ -415,6 +567,9 @@ void free_graph(Graph &g) {
   if (g.fork_ev) cudaEventDestroy(g.fork_ev);
   if (g.join_ev) cudaEventDestroy(g.join_ev);
   if (g.stream2) cudaStreamDestroy(g.stream2);
+  if (g.cold_fork_ev) cudaEventDestroy(g.cold_fork_ev);
+  if (g.cold_join_ev) cudaEventDestroy(g.cold_join_ev);
+  if (g.cold_stream) cudaStreamDestroy(g.cold_stream);
   if (g.stream) cudaStreamDestroy(g.stream);
 }
 
@@ -432,6 +587,9 @@ int build_graph(Graph &g, EdgeSource &edges) {
   }
   MGB_CUDA(cudaEventCreateWithFlags(&g.fork_ev, cudaEventDisableTiming));
   MGB_CUDA(cudaEventCreateWithFlags(&g.join_ev, cudaEventDisableTiming));
+  MGB_CUDA(cudaStreamCreateWithFlags(&g.cold_stream, cudaStreamNonBlocking));
+  MGB_CUDA(cudaEventCreateWithFlags(&g.cold_fork_ev, cudaEventDisableTiming));
+  MGB_CUDA(cudaEventCreateWithFlags(&g.cold_join_ev, cudaEventDisableTiming));
   {
     const char *s = getenv("MGB200_OVERLAP_EPILOGUE");
     g.overlap_epilogue = !(s && s[0] == '0');
@@ -447,6 +605,10 @@ int build_graph(Graph &g, EdgeSource &edges) {
     if ((s = getenv("MGB200_LABELLING")) != nullptr) g.tun.global_order = strcmp(s, "global") == 0;
     if ((s = getenv("MGB200_PUSH_MASK")) != nullptr) g.tun.push_mask = s[0] == '1';
     if ((s = getenv("MGB200_LONE_PARTITION")) != nullptr) g.tun.lone_partition = s[0] == '1';
+    if ((s = getenv("MGB200_TILE_LABELS")) != nullptr)
+      g.tun.tile_labels = static_cast<uint32_t>(std::min<unsigned long>(kMaxTileLabels, strtoul(s, nullptr, 10))) & ~1u;
+    if ((s = getenv("MGB200_TILE_HOT_MB")) != nullptr) g.tun.tile_hot_mb = std::min<uint64_t>(1ull << 20, strtoull(s, nullptr, 10));
+    g.tun.tile_chunk = env_u32("MGB200_TILE_CHUNK", g.tun.tile_chunk);
     if ((s = getenv("MGB200_BARRIER_TIMEOUT_MS")) != nullptr) {
       const unsigned long long ms = strtoull(s, nullptr, 10);
       if (ms) g.tun.barrier_timeout_ms = ms;
@@ -698,6 +860,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     }
     note_mem(g);
     ekey = kb.Current();
+    ekey_alt = kb.Alternate();  // free again: the heavy rows' cold keys are compacted into it
   }
 
   // 6. row pointers over the local rows (uint64)
@@ -713,50 +876,177 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(cudaMemcpyAsync(row_ptr + g.local_rows, &g.local_edges, sizeof(uint64_t), cudaMemcpyHostToDevice, st));
   }
 
-  // 7. heavy class: CSC prefix + segments
+  // 7. heavy class: tile chunks of the hot sources, CSC + segments of the cold ones
   if (g.n_heavy) {
-    MGB_CUDA(cudaMemcpyAsync(&g.heavy_edges, row_ptr + g.n_heavy, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    const uint64_t nh = g.n_heavy;
+    MGB_CUDA(cudaMemcpyAsync(&g.heavy_edges, row_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
+    // 7a. tiles: every owner's hot prefix cut into T-label windows; a window starts on an even label (16-byte aligned)
+    const uint32_t T = weighted ? 0u : g.tun.tile_labels;
+    const uint32_t owners = (g.part_world > 1 && !map.global_order) ? g.part_world : 1u;
+    const TileSet tiles{Dealer{n, owners}, (g.tun.tile_hot_mb << 20) / sizeof(double) / owners};
+    std::vector<uint32_t> t_lo, t_hi, t_base, t_load;
+    for (uint32_t q = 0; T && q < owners; ++q) {
+      const uint64_t s0 = tiles.owners.start(q), end = s0 + std::min(tiles.hot, tiles.owners.count(q));
+      for (uint64_t b = s0 & ~1ull; b < end; b += T) {
+        t_lo.push_back(static_cast<uint32_t>(std::max(b, s0)));
+        t_hi.push_back(static_cast<uint32_t>(std::min(b + T, end)));
+        t_base.push_back(static_cast<uint32_t>(b));
+        t_load.push_back(static_cast<uint32_t>((std::min(b + T, end) - b + 1) & ~1ull));
+      }
+    }
+    const uint32_t nt = static_cast<uint32_t>(t_lo.size());
+    g.n_tiles = nt;
+    const uint64_t pairs = nh * nt;
+    uint32_t *d_lo = nullptr, *d_hi = nullptr, *pair_cnt = nullptr;
+    uint64_t *pair_chunks = nullptr, *pair_chunk_first = nullptr;
+    unsigned long long *tile_chunks = nullptr;
+    if (nt) {
+      MGB_CUDA(tmp.alloc(&d_lo, nt));
+      MGB_CUDA(tmp.alloc(&d_hi, nt));
+      MGB_CUDA(keep_alloc(g, &g.tile_base, nt));
+      MGB_CUDA(keep_alloc(g, &g.tile_load, nt));
+      MGB_CUDA(cudaMemcpyAsync(d_lo, t_lo.data(), nt * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      MGB_CUDA(cudaMemcpyAsync(d_hi, t_hi.data(), nt * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      MGB_CUDA(cudaMemcpyAsync(g.tile_base, t_base.data(), nt * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      MGB_CUDA(cudaMemcpyAsync(g.tile_load, t_load.data(), nt * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      MGB_CUDA(tmp.alloc(&pair_cnt, pairs));
+      MGB_CUDA(tmp.alloc(&pair_chunks, pairs));
+      MGB_CUDA(tmp.alloc(&pair_chunk_first, pairs + 1));
+      MGB_CUDA(tmp.alloc(&tile_chunks, nt));
+      MGB_CUDA(cudaMemsetAsync(tile_chunks, 0, nt * sizeof(unsigned long long), st));
+      tile_pair_kernel<<<blocks_for(pairs, g.sm_count), kThreads, 0, st>>>(nh, nt, row_ptr, ekey, d_lo, d_hi,
+                                                                          g.tun.tile_chunk, pair_cnt, pair_chunks,
+                                                                          tile_chunks);
+      MGB_CUDA(prefix_sum(tmp, pair_chunks, pair_chunk_first, pairs, st));
+    }
+    uint64_t *cold_deg = nullptr, *row_chunks = nullptr, *row_parts = nullptr, *row_cold_segs = nullptr,
+             *cold_seg_first = nullptr;
+    MGB_CUDA(tmp.alloc(&cold_deg, nh));
+    MGB_CUDA(tmp.alloc(&row_chunks, nh));
+    MGB_CUDA(tmp.alloc(&row_parts, nh));
+    MGB_CUDA(tmp.alloc(&row_cold_segs, nh));
+    MGB_CUDA(tmp.alloc(&cold_seg_first, nh + 1));
+    tile_row_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, nt, indeg_local, pair_cnt, pair_chunks,
+                                                                    cold_deg, row_chunks);
+    MGB_CUDA(keep_alloc(g, &g.heavy_ptr, nh + 1));
+    MGB_CUDA(prefix_sum(tmp, cold_deg, g.heavy_ptr, nh, st));
+    uint64_t cold_edges = 0;
+    MGB_CUDA(cudaMemcpyAsync(&cold_edges, g.heavy_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    if (nt) MGB_CUDA(cudaMemcpyAsync(&g.tile_chunks, pair_chunk_first + pairs, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaStreamSynchronize(st));
+    g.tiled_edges = g.heavy_edges - cold_edges;
     if (!getenv("MGB200_SEGMENT_EDGES")) {
       // one warp per segment: aim for >= 8 segments per resident warp (64 warps/SM) so the tail is short
-      // when a partition holds few heavy edges (multi-GPU), capped at 4096 edges
+      // when a partition holds few cold heavy edges (multi-GPU, or most of them tiled), capped at 4096 edges
       const uint64_t resident_warps = static_cast<uint64_t>(g.sm_count) * 64;
-      uint64_t seg = g.heavy_edges / (resident_warps * 8);
+      uint64_t seg = cold_edges / (resident_warps * 8);
       seg = (seg / 256) * 256;
       g.segment_edges = static_cast<uint32_t>(std::min<uint64_t>(4096, std::max<uint64_t>(256, seg)));
     }
-    MGB_CUDA(keep_alloc(g, &g.heavy_ptr, g.n_heavy + 1));
-    MGB_CUDA(cudaMemcpyAsync(g.heavy_ptr, row_ptr, (g.n_heavy + 1) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
-    MGB_CUDA(keep_alloc(g, &g.heavy_idx, g.heavy_edges));
-    low32_kernel<<<blocks_for(g.heavy_edges, g.sm_count), kThreads, 0, st>>>(g.heavy_edges, ekey, idx_flags_heavy,
-                                                                                   g.heavy_idx);
-    if (weighted) {  // rows are sorted, heavy rows first: their weights are the prefix of the sorted weights
+    seg_count_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, cold_deg, row_chunks, g.segment_edges,
+                                                                     row_parts, row_cold_segs);
+    MGB_CUDA(keep_alloc(g, &g.seg_first, nh + 1));
+    MGB_CUDA(prefix_sum(tmp, row_parts, g.seg_first, nh, st));
+    MGB_CUDA(prefix_sum(tmp, row_cold_segs, cold_seg_first, nh, st));
+    MGB_CUDA(cudaMemcpyAsync(&g.n_seg, g.seg_first + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaMemcpyAsync(&g.n_cold_seg, cold_seg_first + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    // 7b. cold edges: the heavy rows' keys without the tiled ones (order kept), as CSC + fixed-size segments
+    const uint64_t *cold_keys = ekey;
+    if (g.tiled_edges) {
+      unsigned long long *d_sel = nullptr;
+      MGB_CUDA(tmp.alloc(&d_sel, 1));
+      size_t bytes = 0;
+      MGB_CUDA(cub::DeviceSelect::If(nullptr, bytes, ekey, ekey_alt, d_sel, static_cast<int64_t>(g.heavy_edges),
+                                     ColdKey{tiles}, st));
+      void *cub_tmp = nullptr;
+      MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+      MGB_CUDA(cub::DeviceSelect::If(cub_tmp, bytes, ekey, ekey_alt, d_sel, static_cast<int64_t>(g.heavy_edges),
+                                     ColdKey{tiles}, st));
+      cold_keys = ekey_alt;
+    }
+    MGB_CUDA(keep_alloc(g, &g.heavy_idx, cold_edges));
+    low32_kernel<<<blocks_for(cold_edges, g.sm_count), kThreads, 0, st>>>(cold_edges, cold_keys, idx_flags_heavy,
+                                                                         g.heavy_idx);
+    if (weighted) {  // rows are sorted, heavy rows first: their weights are the prefix of the sorted weights (no tiles)
       MGB_CUDA(keep_alloc(g, &g.heavy_w, g.heavy_edges));
       MGB_CUDA(cudaMemcpyAsync(g.heavy_w, eval, g.heavy_edges * sizeof(double), cudaMemcpyDeviceToDevice, st));
     }
-    MGB_CUDA(keep_alloc(g, &g.seg_first, g.n_heavy + 1));
-    {
-      cub::TransformInputIterator<uint64_t, SegCount, const uint32_t *> it(indeg_local, SegCount{g.segment_edges});
-      size_t bytes = 0;
-      MGB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, it, g.seg_first, g.n_heavy, st));
-      void *cub_tmp = nullptr;
-      MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
-      MGB_CUDA(cub::DeviceScan::ExclusiveSum(cub_tmp, bytes, it, g.seg_first, g.n_heavy, st));
-    }
-    // total = seg_first[n_heavy-1] + segs(last row)
-    uint64_t last_first = 0;
-    uint32_t last_deg = 0;
-    MGB_CUDA(cudaMemcpyAsync(&last_first, g.seg_first + g.n_heavy - 1, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-    MGB_CUDA(cudaMemcpyAsync(&last_deg, indeg_local + g.n_heavy - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
-    g.n_seg = last_first + (static_cast<uint64_t>(last_deg) + g.segment_edges - 1) / g.segment_edges;
-    MGB_CUDA(cudaMemcpyAsync(g.seg_first + g.n_heavy, &g.n_seg, sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-    MGB_CUDA(keep_alloc(g, &g.seg_row, g.n_seg));
-    MGB_CUDA(keep_alloc(g, &g.seg_begin, g.n_seg));
+    MGB_CUDA(keep_alloc(g, &g.seg_row, g.n_cold_seg));
+    MGB_CUDA(keep_alloc(g, &g.seg_begin, g.n_cold_seg));
+    if (g.tile_chunks) MGB_CUDA(keep_alloc(g, &g.seg_slot, g.n_cold_seg));
     MGB_CUDA(keep_alloc(g, &g.seg_partial, g.n_seg));
-    MGB_CUDA(keep_alloc(g, &g.heavy_sums, g.n_heavy));
-    segment_fill_kernel<<<blocks_for(g.n_heavy * 32, g.sm_count), kThreads, 0, st>>>(
-        g.n_heavy, g.heavy_ptr, g.seg_first, g.segment_edges, g.seg_row, g.seg_begin);
+    MGB_CUDA(keep_alloc(g, &g.heavy_sums, nh));
+    segment_fill_kernel<<<blocks_for(nh * 32, g.sm_count), kThreads, 0, st>>>(
+        nh, g.heavy_ptr, cold_seg_first, g.segment_edges, g.seg_first, g.seg_row, g.seg_begin, g.seg_slot);
+    // 7c. tile chunks -> per tile, SELL-32 slices of chunks sorted by length (ties: row order)
+    if (g.tile_chunks) {
+      std::vector<unsigned long long> per_tile(nt);
+      MGB_CUDA(cudaMemcpyAsync(per_tile.data(), tile_chunks, nt * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      MGB_CUDA(cudaStreamSynchronize(st));
+      std::vector<uint64_t> chunk_first(nt + 1, 0), slice_first(nt + 1, 0);
+      std::vector<uint32_t> slice_tile;
+      for (uint32_t t = 0; t < nt; ++t) {
+        chunk_first[t + 1] = chunk_first[t] + per_tile[t];
+        const uint64_t slices = (per_tile[t] + kSliceRows - 1) / kSliceRows;
+        slice_first[t + 1] = slice_first[t] + slices;
+        slice_tile.insert(slice_tile.end(), slices, t);
+      }
+      const uint64_t ns = slice_first[nt], nc = g.tile_chunks;
+      g.tile_slices = ns;
+      uint64_t *d_chunk_first = nullptr;
+      MGB_CUDA(tmp.alloc(&d_chunk_first, nt + 1));
+      MGB_CUDA(keep_alloc(g, &g.tile_slice_first, nt + 1));
+      MGB_CUDA(keep_alloc(g, &g.tslice_tile, ns));
+      MGB_CUDA(cudaMemcpyAsync(d_chunk_first, chunk_first.data(), (nt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+      MGB_CUDA(cudaMemcpyAsync(g.tile_slice_first, slice_first.data(), (nt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+      MGB_CUDA(cudaMemcpyAsync(g.tslice_tile, slice_tile.data(), ns * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      uint64_t *ckey = nullptr, *ckey_alt = nullptr, *cid = nullptr, *cid_alt = nullptr, *cbegin = nullptr, *cslot = nullptr;
+      uint32_t *clen = nullptr;
+      MGB_CUDA(tmp.alloc(&ckey, nc));
+      MGB_CUDA(tmp.alloc(&ckey_alt, nc));
+      MGB_CUDA(tmp.alloc(&cid, nc));
+      MGB_CUDA(tmp.alloc(&cid_alt, nc));
+      MGB_CUDA(tmp.alloc(&cbegin, nc));
+      MGB_CUDA(tmp.alloc(&clen, nc));
+      MGB_CUDA(tmp.alloc(&cslot, nc));
+      tile_chunk_kernel<<<blocks_for(pairs, g.sm_count), kThreads, 0, st>>>(nh, nt, row_ptr, ekey, d_lo, pair_cnt,
+                                                                           pair_chunk_first, g.seg_first,
+                                                                           g.tun.tile_chunk, ckey, cid, cbegin, clen,
+                                                                           cslot);
+      const uint64_t *sorted_id = nullptr;
+      {  // stable: equal (tile, length) keep row order, so the layout is a function of the graph alone
+        cub::DoubleBuffer<uint64_t> kb(ckey, ckey_alt);
+        cub::DoubleBuffer<uint64_t> vb(cid, cid_alt);
+        size_t bytes = 0;
+        MGB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, kb, vb, nc, 0, 32 + bits_for(nt), st));
+        void *cub_tmp = nullptr;
+        MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+        MGB_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp, bytes, kb, vb, nc, 0, 32 + bits_for(nt), st));
+        sorted_id = vb.Current();
+      }
+      uint64_t *width = nullptr;
+      MGB_CUDA(tmp.alloc(&width, ns));
+      tile_width_kernel<<<blocks_for(ns, g.sm_count), kThreads, 0, st>>>(ns, g.tslice_tile, g.tile_slice_first,
+                                                                        d_chunk_first, sorted_id, clen, width);
+      MGB_CUDA(keep_alloc(g, &g.tslice_colbase, ns + 1));
+      MGB_CUDA(prefix_sum(tmp, width, g.tslice_colbase, ns, st));
+      uint64_t total_cols = 0;
+      MGB_CUDA(cudaMemcpyAsync(&total_cols, g.tslice_colbase + ns, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+      MGB_CUDA(cudaStreamSynchronize(st));
+      MGB_CUDA(keep_alloc(g, &g.tile_idx, total_cols * kSliceRows));
+      MGB_CUDA(keep_alloc(g, &g.tile_slot, ns * kSliceRows));
+      tile_fill_kernel<<<blocks_for(ns * 32, g.sm_count), kThreads, 0, st>>>(
+          ns, g.tslice_tile, g.tile_slice_first, d_chunk_first, g.tile_base, g.tslice_colbase, sorted_id, cbegin, clen,
+          cslot, ekey, static_cast<uint16_t>(T), g.tile_idx, g.tile_slot);
+      // one work item per CTA (one CTA per SM): contiguous slice runs of ~equal cost = columns + 8 per slice
+      g.tile_work = static_cast<uint32_t>(std::min<uint64_t>(ns, g.sm_count));
+      MGB_CUDA(keep_alloc(g, &g.tile_work_begin, static_cast<uint64_t>(g.tile_work) + 1));
+      sell_items_kernel<<<(g.tile_work + 1 + kThreads - 1) / kThreads, kThreads, 0, st>>>(
+          g.tile_work, ns, g.tslice_colbase, total_cols, 8, g.tile_work_begin);
+    }
+    note_mem(g);
   }
 
   // 8. SELL class

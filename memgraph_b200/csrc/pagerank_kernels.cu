@@ -570,12 +570,114 @@ __global__ void __launch_bounds__(kTableThreads, 1) sell_rows_table_kernel(const
 
 // ---- heavy rows: one warp per fixed-size edge segment, then one warp per row ------------------------
 
+// Tile chunks (graph_build.cu 7c): a CTA copies one tile of contrib into shared memory with TMA bulk copies and serves
+// every chunk of that tile from it -- per edge a 2-byte offset and a shared-memory read instead of a 4-byte index and
+// an L2 request.  Slices are tile-major, and each CTA walks ONE contiguous run of them (its work item), so it refills
+// only where its run crosses into the next tile: about (tiles + CTAs) fills per launch.  Inside a tile, the CTA's warps
+// draw slices from a shared counter; a lane adds its chunk in ascending source order and writes the chunk's partial.
+struct TileArgs {
+  const uint16_t *idx;          // [32 * columns] tile offsets, column-major per slice
+  const uint64_t *colbase;      // [slices + 1]
+  const uint32_t *slice_tile;   // [slices]
+  const uint64_t *slot;         // [32 * slices] partial of each lane's chunk, ~0 = padding lane
+  const uint64_t *tile_slice_first;  // [tiles + 1]
+  const uint32_t *tile_base, *tile_load;  // [tiles] first label (even) and labels copied (even)
+  const uint64_t *work_begin;   // [n_work + 1]
+  uint32_t n_work;
+  uint32_t tile_labels;         // T: shared slot T holds the 0.0 every padding offset reads
+  const double *contrib_in;
+  double *seg_partial;
+  IterState *state;
+};
+constexpr int kTileThreads = 512;
+constexpr int kTileUnroll = 16;
+constexpr int kTileEpiCtas = 2;  // CTAs per SM of the side-stream SELL epilogue next to heavy_tiles_kernel
+__device__ __forceinline__ uint16_t ld_index16(const uint16_t *p, uint64_t pol) {
+  uint16_t v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u16 %0, [%1], %2;" : "=h"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__global__ void __launch_bounds__(kTileThreads, 2) heavy_tiles_kernel(const TileArgs a) {  // <= 64 registers
+  extern __shared__ __align__(128) unsigned char tile_smem[];
+  __shared__ __align__(8) unsigned long long fill_bar;
+  __shared__ unsigned long long next_slice;
+  if (ld_volatile_int(&a.state->done)) return;
+  const double *tile = reinterpret_cast<const double *>(tile_smem);
+  const int lane = threadIdx.x & 31;
+  const uint32_t bar = smem_u32(&fill_bar);
+  if (threadIdx.x == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    reinterpret_cast<double *>(tile_smem)[a.tile_labels] = 0.0;  // never overwritten: a fill copies <= T labels
+  }
+  __syncthreads();
+  const uint64_t pol = make_evict_first_policy();
+  uint32_t phase = 0, cur_tile = 0xFFFFFFFFu;
+  for (uint32_t w = blockIdx.x; w < a.n_work; w += gridDim.x) {
+    uint64_t s = a.work_begin[w];
+    const uint64_t s_end = a.work_begin[w + 1];
+    while (s < s_end) {
+      const uint32_t t = a.slice_tile[s];
+      const uint64_t run_end = min(s_end, a.tile_slice_first[t + 1]);
+      if (threadIdx.x == 0) {
+        next_slice = s;
+        if (t != cur_tile) {
+          // the previous tile's shared-memory reads (ordered by the __syncthreads below) precede the async-proxy writes
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          uint64_t keep;
+          asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
+          const uint32_t bytes = a.tile_load[t] * static_cast<uint32_t>(sizeof(double));
+          const unsigned char *src = reinterpret_cast<const unsigned char *>(a.contrib_in + a.tile_base[t]);
+          mbar_expect_tx(bar, bytes);
+          for (uint32_t off = 0; off < bytes; off += 32768u)
+            tma_load_1d(smem_u32(tile_smem + off), src + off, min(32768u, bytes - off), bar, keep);
+        }
+      }
+      __syncthreads();
+      if (t != cur_tile) {
+        mbar_wait(bar, phase);
+        phase ^= 1u;
+        cur_tile = t;
+      }
+      while (true) {
+        unsigned long long my = 0;
+        if (lane == 0) my = atomicAdd(&next_slice, 1ull);
+        my = __shfl_sync(kFull, my, 0);
+        if (my >= run_end) break;
+        const uint64_t c0 = a.colbase[my], ncols = a.colbase[my + 1] - c0;
+        const uint64_t slot = a.slot[my * kSliceRows + lane];
+        const uint16_t *p = a.idx + c0 * kSliceRows + lane;
+        double acc = 0.0;
+        uint16_t nxt[kTileUnroll];
+#pragma unroll
+        for (int j = 0; j < kTileUnroll; ++j)
+          if (static_cast<uint64_t>(j) < ncols) nxt[j] = ld_index16(p + static_cast<size_t>(j) * kSliceRows, pol);
+        for (uint64_t k = 0; k < ncols; k += kTileUnroll) {
+          uint16_t off[kTileUnroll];
+#pragma unroll
+          for (int j = 0; j < kTileUnroll; ++j) off[j] = nxt[j];
+#pragma unroll
+          for (int j = 0; j < kTileUnroll; ++j)  // the next batch of offsets travels while this batch is summed
+            if (k + kTileUnroll + j < ncols) nxt[j] = ld_index16(p + static_cast<size_t>(k + kTileUnroll + j) * kSliceRows, pol);
+#pragma unroll
+          for (int j = 0; j < kTileUnroll; ++j)
+            if (k + j < ncols) acc += tile[off[j]];  // ascending source order inside the chunk
+        }
+        if (slot != ~0ull) a.seg_partial[slot] = acc;
+      }
+      __syncthreads();  // every warp is done with this run (and with next_slice) before the next fill
+      s = run_end;
+    }
+  }
+}
+
 struct HeavyArgs {
   const uint64_t *heavy_ptr;
   const uint32_t *heavy_idx;
   const double *heavy_w;  // edge weights parallel to heavy_idx (weighted variants only)
   const uint32_t *seg_row;
   const uint64_t *seg_begin;
+  const uint64_t *seg_slot;  // partial of each segment (nullptr: identity)
   const uint64_t *seg_first;
   double *seg_partial;
   double *row_sums;  // [n_heavy]
@@ -649,7 +751,7 @@ __global__ void __launch_bounds__(kBlockThreads, MGB_HEAVY_MIN_BLOCKS) heavy_seg
       acc += v1;
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(kFull, acc, o);  // fixed tree
-    if (lane == 0) a.seg_partial[g] = acc;
+    if (lane == 0) a.seg_partial[a.seg_slot ? a.seg_slot[g] : g] = acc;
   }
 }
 
@@ -895,6 +997,50 @@ GatherWindow make_window(const Graph &g) {
   return w;
 }
 
+// the heavy rows' tile chunks: one CTA per work item, one per SM (a tile takes most of the SM's shared memory)
+int launch_heavy_tiles(Graph &g, const double *contrib_in) {
+  if (g.tile_slices == 0) return MGB200_OK;
+  const TileArgs t{g.tile_idx,  g.tslice_colbase, g.tslice_tile,      g.tile_slot, g.tile_slice_first,
+                   g.tile_base, g.tile_load,      g.tile_work_begin,  g.tile_work, g.tun.tile_labels,
+                   contrib_in,  g.seg_partial,    g.state};
+  const int bytes = static_cast<int>((g.tun.tile_labels + 1) * sizeof(double));
+  if (g.tile_attr_bytes < bytes) {
+    MGB_CUDA(cudaFuncSetAttribute(heavy_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    g.tile_attr_bytes = bytes;
+  }
+  heavy_tiles_kernel<<<g.tile_work, kTileThreads, bytes, g.stream>>>(t);
+  MGB_CUDA(cudaGetLastError());
+  return MGB200_OK;
+}
+
+// Heavy-row partials: the tile chunks (shared-memory reads, a 2-byte offset stream) and the cold segments (random HBM
+// gathers) write disjoint partials and wait on different units, so with both present the cold segments run on a stream
+// of their own next to the tile kernel, joined back before the caller's row sums.  The tile kernel goes first: its
+// CTAs need half an SM each and would wait behind a full grid of segment CTAs.
+int launch_heavy_gathers(Graph &g, const HeavyArgs &h, void (*seg_fn)(HeavyArgs), uint64_t seg_grid_cap,
+                         uint64_t *launches) {
+  const bool fork = g.tile_slices > 0 && g.n_cold_seg > 0;
+  if (fork) {  // before the tile kernel: the cold stream waits for the earlier work of the main stream only
+    MGB_CUDA(cudaEventRecord(g.cold_fork_ev, g.stream));
+    MGB_CUDA(cudaStreamWaitEvent(g.cold_stream, g.cold_fork_ev, 0));
+  }
+  const int trc = launch_heavy_tiles(g, h.contrib_in);
+  if (trc) return trc;
+  if (g.tile_slices) ++*launches;
+  if (g.n_cold_seg > 0) {
+    cudaStream_t cs = fork ? g.cold_stream : g.stream;
+    const int grid = static_cast<int>(std::min(seg_grid_cap, ceil_div(g.n_cold_seg, kWarpsPerBlock)));
+    seg_fn<<<grid, kBlockThreads, 0, cs>>>(h);
+    MGB_CUDA(cudaGetLastError());
+    ++*launches;
+    if (fork) {
+      MGB_CUDA(cudaEventRecord(g.cold_join_ev, g.cold_stream));
+      MGB_CUDA(cudaStreamWaitEvent(g.stream, g.cold_join_ev, 0));
+    }
+  }
+  return MGB200_OK;
+}
+
 BarrierArgs make_barrier(const Graph &g) {
   BarrierArgs b{};
   b.state = g.state;
@@ -1059,6 +1205,10 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
     uint64_t egrid_cap = static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(row_epilogue_kernel)));
     if (g.part_world > 1 && g.overlap_epilogue && g.tun.push_ctas > 0)
       egrid_cap = std::min<uint64_t>(egrid_cap, static_cast<uint64_t>(g.sm_count) * g.tun.push_ctas);
+    // the tile kernel needs half an SM's register file next to it (512 threads x 64 registers): at its full grid the
+    // epilogue would hold every SM until it drains and the tile kernel would start only then
+    if (g.overlap_epilogue && g.tile_slices)
+      egrid_cap = std::min<uint64_t>(egrid_cap, static_cast<uint64_t>(g.sm_count) * kTileEpiCtas);
     const int egrid = static_cast<int>(std::min(egrid_cap, ceil_div(g.n_sell, kBlockThreads * kEpiRows)));
     MGB_CUDA(tick(Graph::kClsSellEpi, 0, es));
     row_epilogue_kernel<<<egrid, kBlockThreads, 0, es>>>(s.first_row, s.end_row, g.sell_sums, g.state, ep);
@@ -1073,9 +1223,10 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
     h.heavy_idx = g.heavy_idx;
     h.seg_row = g.seg_row;
     h.seg_begin = g.seg_begin;
+    h.seg_slot = g.seg_slot;
     h.seg_first = g.seg_first;
     h.seg_partial = g.seg_partial;
-    h.n_seg = g.n_seg;
+    h.n_seg = g.n_cold_seg;
     h.n_heavy = g.n_heavy;
     h.segment_edges = g.segment_edges;
     h.contrib_in = contrib_in;
@@ -1085,16 +1236,15 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
     void (*const heavy_fn)(HeavyArgs) = h.window.path == kPathFlags    ? heavy_segments_kernel<kPathFlags>
                                         : h.window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
                                                                        : heavy_segments_kernel<kPathRange>;
-    const void *hfn = reinterpret_cast<const void *>(heavy_fn);
-    uint64_t hgrid_cap = static_cast<uint64_t>(grid_for(g, hfn));
+    uint64_t hgrid_cap = static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_fn)));
     // leave register-file room for the push kernel's CTAs (63 registers x 256 threads each) next to this one
     if (forked && g.part_world > 1 && g.tun.push_ctas > 0 && hgrid_cap > static_cast<uint64_t>(g.sm_count) * 2)
       hgrid_cap -= static_cast<uint64_t>(g.sm_count) * 2;
-    int grid = static_cast<int>(std::min(hgrid_cap, ceil_div(g.n_seg, kWarpsPerBlock)));
     MGB_CUDA(tick(Graph::kClsHeavySeg, 0, g.stream));
-    heavy_fn<<<grid, kBlockThreads, 0, g.stream>>>(h);
+    const int hrc = launch_heavy_gathers(g, h, heavy_fn, hgrid_cap, &launches);
+    if (hrc) return hrc;
     MGB_CUDA(tick(Graph::kClsHeavySeg, 1, g.stream));
-    grid = static_cast<int>(
+    int grid = static_cast<int>(
         std::min(static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_rowsum_kernel))),
                  ceil_div(g.n_heavy, kWarpsPerBlock)));
     MGB_CUDA(tick(Graph::kClsHeavyFin, 0, g.stream));
@@ -1104,7 +1254,6 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
                  ceil_div(g.n_heavy, kBlockThreads * kEpiRows)));
     row_epilogue_kernel<<<grid, kBlockThreads, 0, g.stream>>>(0, g.n_heavy, g.heavy_sums, g.state, ep);
     MGB_CUDA(tick(Graph::kClsHeavyFin, 1, g.stream));
-    ++launches;
     launches += 2;
   }
   if (forked) MGB_CUDA(cudaStreamWaitEvent(g.stream, g.join_ev, 0));
@@ -1169,22 +1318,23 @@ int launch_gather_phase(Graph &g, const double *vec_in, uint64_t *launch_count, 
     h.heavy_w = weighted ? g.heavy_w : nullptr;
     h.seg_row = g.seg_row;
     h.seg_begin = g.seg_begin;
+    h.seg_slot = g.seg_slot;
     h.seg_first = g.seg_first;
     h.seg_partial = g.seg_partial;
-    h.n_seg = g.n_seg;
+    h.n_seg = g.n_cold_seg;
     h.n_heavy = g.n_heavy;
     h.segment_edges = g.segment_edges;
     h.contrib_in = vec_in;
     h.window = window;
     h.state = g.state;
-    void (*const heavy_fn)(HeavyArgs) = (weighted && g.heavy_w)          ? heavy_segments_kernel<kPathRange, true>
+    void (*const heavy_fn)(HeavyArgs) = (weighted && g.heavy_w)        ? heavy_segments_kernel<kPathRange, true>
                                         : window.path == kPathFlags    ? heavy_segments_kernel<kPathFlags>
                                         : window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
                                                                      : heavy_segments_kernel<kPathRange>;
-    const int grid = static_cast<int>(std::min(static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_fn))),
-                                               ceil_div(g.n_seg, kWarpsPerBlock)));
-    heavy_fn<<<grid, kBlockThreads, 0, g.stream>>>(h);
-    ++launches;
+    const int hrc = launch_heavy_gathers(g, h, heavy_fn,  // weighted graphs have no tile class
+                                         static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_fn))),
+                                         &launches);
+    if (hrc) return hrc;
     if (heavy_row_sums) {
       h.row_sums = g.heavy_sums;
       const int rgrid = static_cast<int>(
