@@ -354,7 +354,6 @@ int launch_barrier(Graph &g);
 int launch_sum_and_exchange(Graph &g);
 int launch_write_ranks_original_order(Graph &g, double *d_out);                   // single partition
 int launch_write_ranks_local(Graph &g, double *d_rank_out, uint32_t *d_vertex_out);  // partitioned
-int kernel_occupancy_report(Graph &g, char *buf, size_t cap);
 
 // katz.cu
 struct KatzResult {
@@ -364,9 +363,5 @@ struct KatzResult {
 };
 int katz_iterate(Graph &g, double alpha, double epsilon, uint64_t max_iterations, double *d_out_original_order,
                  KatzResult *res);
-
-// rmat.cu
-int rmat_device(int device, uint32_t scale, uint64_t first_edge, uint64_t count, uint64_t seed, double a, double b,
-                double c, uint32_t *d_from, uint32_t *d_to);
 
 }  // namespace mgb200

@@ -13,7 +13,6 @@
 // 12*E + 24*N (SURVEY 8d).  Per edge: one coalesced 4-byte index read (streamed, evict-first) and
 // one 8-byte gather of contrib[]; per row: rank RMW in place, out-degree read, contrib write.
 #include <algorithm>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 
@@ -997,48 +996,44 @@ GatherWindow make_window(const Graph &g) {
   return w;
 }
 
-// the heavy rows' tile chunks: one CTA per work item, one per SM (a tile takes most of the SM's shared memory)
-int launch_heavy_tiles(Graph &g, const double *contrib_in) {
-  if (g.tile_slices == 0) return MGB200_OK;
-  const TileArgs t{g.tile_idx,  g.tslice_colbase, g.tslice_tile,      g.tile_slot, g.tile_slice_first,
-                   g.tile_base, g.tile_load,      g.tile_work_begin,  g.tile_work, g.tun.tile_labels,
-                   contrib_in,  g.seg_partial,    g.state};
-  const int bytes = static_cast<int>((g.tun.tile_labels + 1) * sizeof(double));
-  if (g.tile_attr_bytes < bytes) {
-    MGB_CUDA(cudaFuncSetAttribute(heavy_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    g.tile_attr_bytes = bytes;
-  }
-  heavy_tiles_kernel<<<g.tile_work, kTileThreads, bytes, g.stream>>>(t);
-  MGB_CUDA(cudaGetLastError());
-  return MGB200_OK;
+// The only places that fill the gather kernels' arguments from a graph; `vec` is the gathered vector (slot n holds 0),
+// `weighted` multiplies every gathered value by its edge weight (one partition only, see launch_gather_phase).
+SellArgs make_sell_args(const Graph &g, const double *vec, const GatherWindow &window, bool weighted) {
+  SellArgs s{};
+  s.colbase = g.sell_colbase;
+  s.idx = g.sell_idx;
+  s.w = weighted ? g.sell_w : nullptr;
+  s.work = g.sell_work_items;
+  s.n_work = g.sell_work;
+  s.queue = g.queue;
+  s.mode = g.sell_static ? 1u : 0u;
+  s.first_row = g.n_heavy;
+  s.end_row = g.n_heavy + g.n_sell;
+  s.contrib_in = vec;
+  s.window = window;
+  s.state = g.state;
+  s.sums = g.sell_sums;
+  return s;
 }
 
-// Heavy-row partials: the tile chunks (shared-memory reads, a 2-byte offset stream) and the cold segments (random HBM
-// gathers) write disjoint partials and wait on different units, so with both present the cold segments run on a stream
-// of their own next to the tile kernel, joined back before the caller's row sums.  The tile kernel goes first: its
-// CTAs need half an SM each and would wait behind a full grid of segment CTAs.
-int launch_heavy_gathers(Graph &g, const HeavyArgs &h, void (*seg_fn)(HeavyArgs), uint64_t seg_grid_cap,
-                         uint64_t *launches) {
-  const bool fork = g.tile_slices > 0 && g.n_cold_seg > 0;
-  if (fork) {  // before the tile kernel: the cold stream waits for the earlier work of the main stream only
-    MGB_CUDA(cudaEventRecord(g.cold_fork_ev, g.stream));
-    MGB_CUDA(cudaStreamWaitEvent(g.cold_stream, g.cold_fork_ev, 0));
-  }
-  const int trc = launch_heavy_tiles(g, h.contrib_in);
-  if (trc) return trc;
-  if (g.tile_slices) ++*launches;
-  if (g.n_cold_seg > 0) {
-    cudaStream_t cs = fork ? g.cold_stream : g.stream;
-    const int grid = static_cast<int>(std::min(seg_grid_cap, ceil_div(g.n_cold_seg, kWarpsPerBlock)));
-    seg_fn<<<grid, kBlockThreads, 0, cs>>>(h);
-    MGB_CUDA(cudaGetLastError());
-    ++*launches;
-    if (fork) {
-      MGB_CUDA(cudaEventRecord(g.cold_join_ev, g.cold_stream));
-      MGB_CUDA(cudaStreamWaitEvent(g.stream, g.cold_join_ev, 0));
-    }
-  }
-  return MGB200_OK;
+HeavyArgs make_heavy_args(const Graph &g, const double *vec, const GatherWindow &window, bool weighted) {
+  HeavyArgs h{};
+  h.heavy_ptr = g.heavy_ptr;
+  h.heavy_idx = g.heavy_idx;
+  h.heavy_w = weighted ? g.heavy_w : nullptr;
+  h.seg_row = g.seg_row;
+  h.seg_begin = g.seg_begin;
+  h.seg_slot = g.seg_slot;
+  h.seg_first = g.seg_first;
+  h.seg_partial = g.seg_partial;
+  h.row_sums = g.heavy_sums;
+  h.n_seg = g.n_cold_seg;
+  h.n_heavy = g.n_heavy;
+  h.segment_edges = g.segment_edges;
+  h.contrib_in = vec;
+  h.window = window;
+  h.state = g.state;
+  return h;
 }
 
 BarrierArgs make_barrier(const Graph &g) {
@@ -1107,6 +1102,83 @@ int launch_sell_rows(Graph &g, const SellArgs &s) {
   return MGB200_OK;
 }
 
+// The same SELL rows through the TMA index ring + LDGSTS gathers (opt-in MGB200_SELL_KERNEL=stream, sell_stream.cuh)
+int launch_sell_stream(Graph &g, const SellArgs &s) {
+  if (!g.stream_attr_set) {  // per device, so per graph handle
+    MGB_CUDA(cudaFuncSetAttribute(sell_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStreamSmemBytes));
+    g.stream_attr_set = true;
+  }
+  SellStreamArgs t{};
+  t.colbase = s.colbase;
+  t.idx = s.idx;
+  t.item_begin = g.sell_item_begin;
+  t.n_items = g.sell_items;
+  t.first_row = s.first_row;
+  t.end_row = s.end_row;
+  t.contrib_in = s.contrib_in;
+  t.window = s.window;
+  t.state = s.state;
+  t.sums = s.sums;
+  const int grid = static_cast<int>(std::min<uint64_t>(g.sm_count, ceil_div(g.sell_items, kStreamWarps)));
+  sell_stream_kernel<<<grid, kStreamThreads, kStreamSmemBytes, g.stream>>>(t);
+  MGB_CUDA(cudaGetLastError());
+  return MGB200_OK;
+}
+
+// Heavy-row partials: the tile chunks (shared-memory reads, a 2-byte offset stream; one CTA per work item, one per SM,
+// as a tile takes most of the SM's shared memory) and the cold segments (random HBM gathers) write disjoint partials
+// and wait on different units, so with both present the cold segments run on a stream of their own next to the tile
+// kernel, joined back before the caller's row sums.  The tile kernel goes first: its CTAs need half an SM each and
+// would wait behind a full grid of segment CTAs.  The segment grid leaves `reserve_ctas` CTA slots to other kernels.
+int launch_heavy_partials(Graph &g, const HeavyArgs &h, uint64_t reserve_ctas, uint64_t *launches) {
+  void (*const seg_fn)(HeavyArgs) = h.heavy_w != nullptr           ? heavy_segments_kernel<kPathRange, true>
+                                    : h.window.path == kPathFlags  ? heavy_segments_kernel<kPathFlags>
+                                    : h.window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
+                                                                   : heavy_segments_kernel<kPathRange>;
+  uint64_t seg_grid_cap = static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(seg_fn)));
+  if (seg_grid_cap > reserve_ctas) seg_grid_cap -= reserve_ctas;
+  const bool fork = g.tile_slices > 0 && g.n_cold_seg > 0;
+  if (fork) {  // before the tile kernel: the cold stream waits for the earlier work of the main stream only
+    MGB_CUDA(cudaEventRecord(g.cold_fork_ev, g.stream));
+    MGB_CUDA(cudaStreamWaitEvent(g.cold_stream, g.cold_fork_ev, 0));
+  }
+  if (g.tile_slices > 0) {
+    const TileArgs t{g.tile_idx,   g.tslice_colbase, g.tslice_tile,     g.tile_slot, g.tile_slice_first,
+                     g.tile_base,  g.tile_load,      g.tile_work_begin, g.tile_work, g.tun.tile_labels,
+                     h.contrib_in, g.seg_partial,    g.state};
+    const int bytes = static_cast<int>((g.tun.tile_labels + 1) * sizeof(double));
+    if (g.tile_attr_bytes < bytes) {
+      MGB_CUDA(cudaFuncSetAttribute(heavy_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+      g.tile_attr_bytes = bytes;
+    }
+    heavy_tiles_kernel<<<g.tile_work, kTileThreads, bytes, g.stream>>>(t);
+    MGB_CUDA(cudaGetLastError());
+    ++*launches;
+  }
+  if (g.n_cold_seg > 0) {
+    cudaStream_t cs = fork ? g.cold_stream : g.stream;
+    const int grid = static_cast<int>(std::min(seg_grid_cap, ceil_div(g.n_cold_seg, kWarpsPerBlock)));
+    seg_fn<<<grid, kBlockThreads, 0, cs>>>(h);
+    MGB_CUDA(cudaGetLastError());
+    ++*launches;
+    if (fork) {
+      MGB_CUDA(cudaEventRecord(g.cold_join_ev, g.cold_stream));
+      MGB_CUDA(cudaStreamWaitEvent(g.stream, g.cold_join_ev, 0));
+    }
+  }
+  return MGB200_OK;
+}
+
+// per heavy row: its partials summed in segment order into h.row_sums
+int launch_heavy_rowsums(Graph &g, const HeavyArgs &h) {
+  const int grid = static_cast<int>(
+      std::min(static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_rowsum_kernel))),
+               ceil_div(g.n_heavy, kWarpsPerBlock)));
+  heavy_rowsum_kernel<<<grid, kBlockThreads, 0, g.stream>>>(h);
+  MGB_CUDA(cudaGetLastError());
+  return MGB200_OK;
+}
+
 int launch_init(Graph &g, const IterateConfig &cfg) {
   MGB_CUDA(cudaSetDevice(g.device));
   const int grid = grid_for(g, reinterpret_cast<const void *>(init_kernel));
@@ -1133,6 +1205,7 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
                      uint64_t *spmv_count) {
   const RowEpilogue ep = make_epilogue(g, it, cfg);
   const double *contrib_in = g.contrib(static_cast<int>(it & 1ull));
+  const GatherWindow window = make_window(g);
   uint64_t launches = 0;
   const bool timed = g.time_spmv && g.timed_launches < Graph::kMaxTimedLaunches;
   auto tick = [&](int cls, int edge, cudaStream_t st) -> cudaError_t {
@@ -1148,47 +1221,11 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
   }
   bool forked = false;
   if (g.n_slices > 0) {
-    SellArgs s{};
-    s.colbase = g.sell_colbase;
-    s.idx = g.sell_idx;
-    s.work = g.sell_work_items;
-    s.n_work = g.sell_work;
-    s.queue = g.queue;
-    s.mode = g.sell_static ? 1u : 0u;
-    s.first_row = g.n_heavy;
-    s.end_row = g.n_heavy + g.n_sell;
-    s.contrib_in = contrib_in;
-    s.window = make_window(g);
-    s.state = g.state;
-    s.sums = g.sell_sums;
-    // "rows" (default): ticketed warp-per-slice kernel, gathers through LDG; "stream": TMA index ring + LDGSTS gathers
-    // (sell_stream.cuh) -- correct, but slower than the LDG kernel (sell_stream.cuh)
-    const bool stream_kernel = g.tun.stream_kernel && g.sell_items > 0;
+    const SellArgs s = make_sell_args(g, contrib_in, window, false);
     cudaStream_t es = g.overlap_epilogue ? g.stream2 : g.stream;
     MGB_CUDA(tick(Graph::kClsSell, 0, g.stream));
-    if (stream_kernel) {
-      if (!g.stream_attr_set) {  // per device, so per graph handle
-        MGB_CUDA(cudaFuncSetAttribute(sell_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      kStreamSmemBytes));
-        g.stream_attr_set = true;
-      }
-      SellStreamArgs t{};
-      t.colbase = g.sell_colbase;
-      t.idx = g.sell_idx;
-      t.item_begin = g.sell_item_begin;
-      t.n_items = g.sell_items;
-      t.first_row = s.first_row;
-      t.end_row = s.end_row;
-      t.contrib_in = contrib_in;
-      t.window = s.window;
-      t.state = g.state;
-      t.sums = g.sell_sums;
-      const int sgrid = static_cast<int>(std::min<uint64_t>(g.sm_count, ceil_div(g.sell_items, kStreamWarps)));
-      sell_stream_kernel<<<sgrid, kStreamThreads, kStreamSmemBytes, g.stream>>>(t);
-    } else {
-      const int rc = launch_sell_rows(g, s);
-      if (rc) return rc;
-    }
+    const int rc = (g.tun.stream_kernel && g.sell_items > 0) ? launch_sell_stream(g, s) : launch_sell_rows(g, s);
+    if (rc) return rc;
     ++launches;
     MGB_CUDA(tick(Graph::kClsSell, 1, g.stream));
     // the epilogue (+ NVLink push to the peers) of the SELL rows runs on the side stream, next to the heavy-row kernels
@@ -1218,38 +1255,18 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
     if (spmv_count) *spmv_count += 1;
   }
   if (g.n_seg > 0) {
-    HeavyArgs h{};
-    h.heavy_ptr = g.heavy_ptr;
-    h.heavy_idx = g.heavy_idx;
-    h.seg_row = g.seg_row;
-    h.seg_begin = g.seg_begin;
-    h.seg_slot = g.seg_slot;
-    h.seg_first = g.seg_first;
-    h.seg_partial = g.seg_partial;
-    h.n_seg = g.n_cold_seg;
-    h.n_heavy = g.n_heavy;
-    h.segment_edges = g.segment_edges;
-    h.contrib_in = contrib_in;
-    h.window = make_window(g);
-    h.row_sums = g.heavy_sums;
-    h.state = g.state;
-    void (*const heavy_fn)(HeavyArgs) = h.window.path == kPathFlags    ? heavy_segments_kernel<kPathFlags>
-                                        : h.window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
-                                                                       : heavy_segments_kernel<kPathRange>;
-    uint64_t hgrid_cap = static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_fn)));
-    // leave register-file room for the push kernel's CTAs (63 registers x 256 threads each) next to this one
-    if (forked && g.part_world > 1 && g.tun.push_ctas > 0 && hgrid_cap > static_cast<uint64_t>(g.sm_count) * 2)
-      hgrid_cap -= static_cast<uint64_t>(g.sm_count) * 2;
+    const HeavyArgs h = make_heavy_args(g, contrib_in, window, false);
+    // leave register-file room for the push kernel's CTAs (63 registers x 256 threads each) next to the segment kernel
+    const uint64_t reserve_ctas =
+        (forked && g.part_world > 1 && g.tun.push_ctas > 0) ? static_cast<uint64_t>(g.sm_count) * 2 : 0;
     MGB_CUDA(tick(Graph::kClsHeavySeg, 0, g.stream));
-    const int hrc = launch_heavy_gathers(g, h, heavy_fn, hgrid_cap, &launches);
-    if (hrc) return hrc;
+    int rc = launch_heavy_partials(g, h, reserve_ctas, &launches);
+    if (rc) return rc;
     MGB_CUDA(tick(Graph::kClsHeavySeg, 1, g.stream));
-    int grid = static_cast<int>(
-        std::min(static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_rowsum_kernel))),
-                 ceil_div(g.n_heavy, kWarpsPerBlock)));
     MGB_CUDA(tick(Graph::kClsHeavyFin, 0, g.stream));
-    heavy_rowsum_kernel<<<grid, kBlockThreads, 0, g.stream>>>(h);
-    grid = static_cast<int>(
+    rc = launch_heavy_rowsums(g, h);
+    if (rc) return rc;
+    const int grid = static_cast<int>(
         std::min(static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(row_epilogue_kernel))),
                  ceil_div(g.n_heavy, kBlockThreads * kEpiRows)));
     row_epilogue_kernel<<<grid, kBlockThreads, 0, g.stream>>>(0, g.n_heavy, g.heavy_sums, g.state, ep);
@@ -1293,54 +1310,17 @@ int launch_gather_phase(Graph &g, const double *vec_in, uint64_t *launch_count, 
     return MGB200_ERR_INVALID_ARGUMENT;
   }
   if (g.n_slices > 0) {
-    SellArgs s{};
-    s.colbase = g.sell_colbase;
-    s.idx = g.sell_idx;
-    s.w = weighted ? g.sell_w : nullptr;
-    s.work = g.sell_work_items;
-    s.n_work = g.sell_work;
-    s.queue = g.queue;
-    s.mode = g.sell_static ? 1u : 0u;
-    s.first_row = g.n_heavy;
-    s.end_row = g.n_heavy + g.n_sell;
-    s.contrib_in = vec_in;
-    s.window = window;
-    s.state = g.state;
-    s.sums = g.sell_sums;
-    const int rc = launch_sell_rows(g, s);
+    const int rc = launch_sell_rows(g, make_sell_args(g, vec_in, window, weighted));
     if (rc) return rc;
     ++launches;
   }
   if (g.n_seg > 0) {
-    HeavyArgs h{};
-    h.heavy_ptr = g.heavy_ptr;
-    h.heavy_idx = g.heavy_idx;
-    h.heavy_w = weighted ? g.heavy_w : nullptr;
-    h.seg_row = g.seg_row;
-    h.seg_begin = g.seg_begin;
-    h.seg_slot = g.seg_slot;
-    h.seg_first = g.seg_first;
-    h.seg_partial = g.seg_partial;
-    h.n_seg = g.n_cold_seg;
-    h.n_heavy = g.n_heavy;
-    h.segment_edges = g.segment_edges;
-    h.contrib_in = vec_in;
-    h.window = window;
-    h.state = g.state;
-    void (*const heavy_fn)(HeavyArgs) = (weighted && g.heavy_w)        ? heavy_segments_kernel<kPathRange, true>
-                                        : window.path == kPathFlags    ? heavy_segments_kernel<kPathFlags>
-                                        : window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
-                                                                     : heavy_segments_kernel<kPathRange>;
-    const int hrc = launch_heavy_gathers(g, h, heavy_fn,  // weighted graphs have no tile class
-                                         static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_fn))),
-                                         &launches);
-    if (hrc) return hrc;
+    const HeavyArgs h = make_heavy_args(g, vec_in, window, weighted);  // weighted graphs have no tile class
+    int rc = launch_heavy_partials(g, h, 0, &launches);
+    if (rc) return rc;
     if (heavy_row_sums) {
-      h.row_sums = g.heavy_sums;
-      const int rgrid = static_cast<int>(
-          std::min(static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(heavy_rowsum_kernel))),
-                   ceil_div(g.n_heavy, kWarpsPerBlock)));
-      heavy_rowsum_kernel<<<rgrid, kBlockThreads, 0, g.stream>>>(h);
+      rc = launch_heavy_rowsums(g, h);
+      if (rc) return rc;
       ++launches;
     }
   }
@@ -1375,16 +1355,6 @@ int launch_write_ranks_local(Graph &g, double *d_rank_out, uint32_t *d_vertex_ou
   write_local_kernel<<<grid, kBlockThreads, 0, g.stream>>>(g.local_rows, g.rank, g.local_vertex, g.state,
                                                            d_rank_out, d_vertex_out);
   MGB_CUDA(cudaGetLastError());
-  return MGB200_OK;
-}
-
-int kernel_occupancy_report(Graph &g, char *buf, size_t cap) {
-  int a = 0, b = 0, c = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, sell_rows_kernel<kPathRange>, kBlockThreads, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, heavy_segments_kernel<kPathRange>, kBlockThreads, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, heavy_rowsum_kernel, kBlockThreads, 0);
-  snprintf(buf, cap, "sm=%d blocks/SM: sell=%d heavy_seg=%d heavy_fin=%d (block=%d threads)", g.sm_count, a, b, c,
-           kBlockThreads);
   return MGB200_OK;
 }
 

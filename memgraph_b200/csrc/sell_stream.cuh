@@ -10,8 +10,9 @@
 //              batch of 8 columns per commit group, kVals batches deep, no registers held
 //   3. reduce: the lane adds its own landed values in column order (fixed order => deterministic) and
 //              stores the row sum at a slice boundary (the epilogue is sell_epilogue_kernel, as for the rows kernel)
-// Parity-green, but slower than the LDG kernel at scale-26: the divergent 8-byte LDGSTS costs more per sector in
-// L1TEX than LDG, and deeper rings make it worse.
+// Parity-green.  It was slower than the LDG kernel at scale-26 on the GPU it was written for: the divergent 8-byte
+// LDGSTS costs more per sector in L1TEX than LDG, and deeper rings make it worse.  On the H100 it runs within 1 % of
+// the LDG kernel (DESIGN.md §4).
 // The TMA ring is the right tool for the contiguous index stream; the gather is better left to LDG.
 #pragma once
 
