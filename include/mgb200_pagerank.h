@@ -67,6 +67,9 @@ typedef struct mgb200_graph_info {
   uint64_t build_peak_bytes; /* device memory in use at the build's high-water mark   */
   uint64_t tiled_edges;    /* heavy-row edges gathered from shared-memory tiles       */
   uint64_t tile_chunks;    /* their (row, tile) runs of <= MGB200_TILE_CHUNK edges    */
+  uint64_t block_edges;    /* in-edges from labels >= MGB200_BLOCK_FROM (block class) */
+  uint64_t block_chunks;   /* their (row, label block) runs, <= MGB200_BLOCK_CHUNK    */
+  uint64_t blocks;         /* label blocks with at least one chunk (one launch each)  */
 } mgb200_graph_info;
 
 typedef struct mgb200_run_stats {

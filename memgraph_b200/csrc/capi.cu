@@ -614,6 +614,9 @@ int mgb200_graph_get_info(const mgb200_graph *h, mgb200_graph_info *info) {
   info->build_peak_bytes = g.build_peak_bytes;
   info->tiled_edges = g.tiled_edges;
   info->tile_chunks = g.tile_chunks;
+  info->block_edges = g.block_edges;
+  info->block_chunks = g.block_chunks;
+  info->blocks = g.block_slice_first.empty() ? 0 : g.block_slice_first.size() - 1;
   return MGB200_OK;
 }
 

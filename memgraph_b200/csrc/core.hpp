@@ -31,6 +31,7 @@ constexpr uint32_t kIdxL2Hot = 0x80000000u;     // keep in L2 (evict_last), else
 constexpr uint32_t kIdxL1Hot = 0x40000000u;     // may allocate in L1, else bypass
 constexpr uint32_t kIdxLabelMask = 0x3FFFFFFFu; // the label itself: flagged graphs have n < 2^30
 constexpr uint32_t kNoL1Hints = 0xFFFFFFFFu;    // l1_hot_labels() when MGB200_L1_HOT_K < 0
+constexpr uint64_t kMaxBlocks = 4096;           // most label blocks (= block-pass launches per gather) of one graph
 
 // Which labels a partition owns and how its local rows (ascending label) map onto them.
 //   dealt ranges (default): sorted position p -> owner p % P, label = start(owner) + p / P.  Every partition owns ONE
@@ -166,8 +167,9 @@ struct Graph {
                                     // row's contribution (has an in-edge from it); nullptr = push to every peer
 
   // heavy class.  A heavy row's in-edges are split at the tile boundary (graph_build.cu TileSet): sources in the tiled
-  // hot prefix are summed from shared-memory tiles of contrib (tile chunks), the rest (cold edges) by edge segments.
-  // Row r owns partials [seg_first[r], seg_first[r + 1]): its tile chunks in tile order, then its cold segments.
+  // hot prefix are summed from shared-memory tiles of contrib (tile chunks), the rest (cold edges) by edge segments,
+  // except those in the block class (below).  Row r owns partials [seg_first[r], seg_first[r + 1]): its tile chunks in
+  // tile order, then its cold segments, then its block chunks.
   uint64_t heavy_edges = 0;       // all in-edges of the heavy rows (tiled + cold)
   uint64_t *heavy_ptr = nullptr;  // [n_heavy + 1] over the cold edges
   uint32_t *heavy_idx = nullptr;  // [cold edges] source labels (+ hot flags if idx_flagged), ascending inside a row
@@ -196,6 +198,20 @@ struct Graph {
   uint32_t tile_work = 0;               // work items = CTAs of heavy_tiles_kernel: contiguous slice runs, ~equal cost
   uint64_t *tile_work_begin = nullptr;  // [tile_work + 1]
   int tile_attr_bytes = 0;              // dynamic shared memory already granted to heavy_tiles_kernel
+  // block class (one partition, unweighted; graph_build.cu steps 6b and 9).  A heavy row's in-edges from labels >=
+  // block_from are summed one label block of block_labels labels at a time, so the block's part of contrib stays in L2
+  // for its whole pass.  A block chunk is <= block_chunk consecutive edges of one heavy row whose sources lie in one
+  // block; per block the chunks are sorted by length and stored as SELL-32 slices of 32-bit labels (padding = label
+  // n -> 0.0), one partial slot per lane.  A heavy row's partials: tile chunks, CSC segments, then block chunks in
+  // block order.
+  uint64_t block_edges = 0, block_chunks = 0;
+  uint64_t block_labels = 0;                // labels per block (MGB200_BLOCK_LABELS, raised to keep <= kMaxBlocks)
+  uint64_t block_slices = 0;
+  std::vector<uint64_t> block_slice_first;  // host: [launched blocks + 1], empty blocks skipped
+  std::vector<uint32_t> block_lo;           // host: [launched blocks] first label of each launched block
+  uint64_t *bslice_colbase = nullptr;       // [block_slices + 1] in units of 32-entry columns
+  uint32_t *block_idx = nullptr;            // [32 * columns] source labels, pad = n
+  uint64_t *block_slot = nullptr;           // [32 * block_slices] partial written by each lane; ~0 = padding lane
   double *heavy_sums = nullptr;   // [n_heavy] per-row gathered sums of the current iteration
   // optional edge weights (cuGraph-semantics variants only; one partition): parallel to heavy_idx / sell_idx, pad = 0
   double *heavy_w = nullptr, *sell_w = nullptr;
@@ -268,6 +284,10 @@ struct Graph {
     uint32_t tile_labels = 16384;  // MGB200_TILE_LABELS: labels per shared-memory tile (even, <= kMaxTileLabels; 0 = off)
     uint64_t tile_hot_mb = 16;     // MGB200_TILE_HOT_MB: tiled prefix of contrib (split between the owners like L2_HOT_MB)
     uint32_t tile_chunk = 256;     // MGB200_TILE_CHUNK: most edges of one tile chunk
+    uint64_t block_from = 2u << 20;    // MGB200_BLOCK_FROM: first label of the block class (16 MB of contrib)
+    uint64_t block_labels = 2u << 20;  // MGB200_BLOCK_LABELS: labels per block (0 = off)
+    uint32_t block_chunk = 16;         // MGB200_BLOCK_CHUNK: most edges of one block chunk (DESIGN.md §4: a pass lasts
+                                       // as long as its longest chunk's chain of dependent gathers)
     unsigned long long barrier_timeout_ms = 20000;  // MGB200_BARRIER_TIMEOUT_MS
   } tun;
   // hot thresholds in LOCAL label units (label - first label of the owning partition); one definition for the

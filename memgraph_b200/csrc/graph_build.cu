@@ -227,9 +227,17 @@ struct TileSet {
     return label - s0 < hot;
   }
 };
-struct ColdKey {  // cub::DeviceSelect predicate: the edge's source is not tiled
+struct ColdKey {  // cub::DeviceSelect predicate: the edge's source is neither tiled nor in the block class
   TileSet ts;
-  __device__ bool operator()(uint64_t key) const { return !ts.hot_label(static_cast<uint32_t>(key)); }
+  uint64_t block_from;  // first label of the block class (n + 1 without one)
+  __device__ bool operator()(uint64_t key) const {
+    const uint32_t src = static_cast<uint32_t>(key);
+    return src < block_from && !ts.hot_label(src);
+  }
+};
+struct BlockKey {  // cub::DeviceSelect predicate: the edge's source is in the block class
+  uint64_t block_from;
+  __device__ bool operator()(uint64_t key) const { return static_cast<uint32_t>(key) >= block_from; }
 };
 
 __device__ __forceinline__ uint64_t lower_bound_key(const uint64_t *key, uint64_t lo, uint64_t hi, uint64_t v) {
@@ -262,7 +270,8 @@ __global__ void tile_pair_kernel(uint64_t n_heavy, uint32_t n_tiles, const uint6
 
 // per heavy row: cold in-degree and tile chunks (no tiles: the in-degree and 0)
 __global__ void tile_row_kernel(uint64_t n_heavy, uint32_t n_tiles, const uint32_t *indeg_local, const uint32_t *pair_cnt,
-                                const uint64_t *pair_chunks, uint64_t *cold_deg, uint64_t *row_chunks) {
+                                const uint64_t *pair_chunks, const uint64_t *block_ptr, uint64_t *cold_deg,
+                                uint64_t *row_chunks) {
   const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
   for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n_heavy; r += stride) {
     uint64_t hot = 0, chunks = 0;
@@ -270,18 +279,24 @@ __global__ void tile_row_kernel(uint64_t n_heavy, uint32_t n_tiles, const uint32
       hot += pair_cnt[r * n_tiles + t];
       chunks += pair_chunks[r * n_tiles + t];
     }
-    cold_deg[r] = indeg_local[r] - hot;
+    cold_deg[r] = indeg_local[r] - hot - (block_ptr ? block_ptr[r + 1] - block_ptr[r] : 0);  // block edges excluded
     row_chunks[r] = chunks;
   }
 }
 
-// per heavy row: partials (tile chunks + cold segments) and cold segments
+// block chunks of local row r: [chunk_first[block_ptr[r]], chunk_first[block_ptr[r + 1]])
+__device__ __forceinline__ uint64_t row_block_chunks(const uint64_t *block_ptr, const uint64_t *chunk_first, uint64_t r) {
+  return block_ptr ? chunk_first[block_ptr[r + 1]] - chunk_first[block_ptr[r]] : 0;
+}
+
+// per heavy row: partials (tile chunks + cold segments + block chunks) and cold segments
 __global__ void seg_count_kernel(uint64_t n_heavy, const uint64_t *cold_deg, const uint64_t *row_chunks,
-                                 uint32_t seg_edges, uint64_t *row_parts, uint64_t *row_cold_segs) {
+                                 const uint64_t *block_ptr, const uint64_t *block_chunk_first, uint32_t seg_edges,
+                                 uint64_t *row_parts, uint64_t *row_cold_segs) {
   const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
   for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n_heavy; r += stride) {
     const uint64_t segs = (cold_deg[r] + seg_edges - 1) / seg_edges;
-    row_parts[r] = row_chunks[r] + segs;
+    row_parts[r] = row_chunks[r] + segs + row_block_chunks(block_ptr, block_chunk_first, r);
     row_cold_segs[r] = segs;
   }
 }
@@ -355,17 +370,21 @@ __global__ void tile_fill_kernel(uint64_t n_slices, const uint32_t *slice_tile, 
 }
 
 __global__ void segment_fill_kernel(uint64_t n_heavy, const uint64_t *heavy_ptr, const uint64_t *cold_seg_first,
-                                    uint32_t seg_edges, const uint64_t *seg_first, uint32_t *seg_row, uint64_t *seg_begin, uint64_t *seg_slot) {
-  // one warp per heavy row; lanes stride over that row's cold segments, which follow its tile chunks in partial order
+                                    uint32_t seg_edges, const uint64_t *seg_first, const uint64_t *block_ptr,
+                                    const uint64_t *block_chunk_first, uint32_t *seg_row, uint64_t *seg_begin,
+                                    uint64_t *seg_slot) {
+  // one warp per heavy row; lanes stride over that row's cold segments, which follow its tile chunks and precede its
+  // block chunks in partial order
   const int lane = threadIdx.x & 31;
   const uint64_t warps_total = static_cast<uint64_t>(gridDim.x) * (blockDim.x >> 5);
   for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n_heavy;
        r += warps_total) {
     const uint64_t s0 = cold_seg_first[r], s1 = cold_seg_first[r + 1], e0 = heavy_ptr[r];
+    const uint64_t end = seg_first[r + 1] - row_block_chunks(block_ptr, block_chunk_first, r);
     for (uint64_t s = s0 + lane; s < s1; s += 32) {
       seg_row[s] = static_cast<uint32_t>(r);
       seg_begin[s] = e0 + (s - s0) * seg_edges;
-      if (seg_slot) seg_slot[s] = seg_first[r + 1] - (s1 - s);  // the row's partials end with its cold segments
+      if (seg_slot) seg_slot[s] = end - (s1 - s);
     }
   }
 }
@@ -402,6 +421,88 @@ __global__ void sell_fill_kernel(uint64_t n_slices, uint64_t first_row, uint64_t
       double *wd = sell_w + c0 * kSliceRows + lane;
       for (uint32_t k = 0; k < width; ++k) wd[static_cast<size_t>(k) * kSliceRows] = k < deg ? w_sorted[e0 + k] : 0.0;
     }
+  }
+}
+
+// ---- block class ------------------------------------------------------------------------------------------
+
+// per heavy row: the number of block edges (the tail of its ascending sources from `from` on)
+__global__ void block_row_kernel(uint64_t rows, const uint64_t *row_ptr, const uint64_t *key, uint64_t from,
+                                 uint64_t *block_cnt) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t r = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < rows; r += stride)
+    block_cnt[r] = row_ptr[r + 1] - lower_bound_key(key, row_ptr[r], row_ptr[r + 1], (r << 32) | from);
+}
+
+// 1 where a block edge (compacted keys, row-major, ascending sources) starts a chunk: every `chunk`-th edge of a
+// row's run of sources in one block
+__global__ void block_start_kernel(uint64_t count, const uint64_t *bkey, const uint64_t *block_ptr, uint64_t from,
+                                   uint64_t labels, uint32_t chunk, uint64_t *start) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += stride) {
+    const uint64_t k = bkey[i], r = k >> 32, b = (static_cast<uint32_t>(k) - from) / labels;
+    const uint64_t first = block_ptr[r];
+    bool st = i == first || (static_cast<uint32_t>(bkey[i - 1]) - from) / labels != b;
+    if (!st) st = (i - lower_bound_key(bkey, first, i, (r << 32) | (from + b * labels))) % chunk == 0;
+    start[i] = st;
+  }
+}
+
+// one record per chunk, in (row, block) order: first edge, row, per-block count
+__global__ void block_chunk_kernel(uint64_t count, const uint64_t *bkey, const uint64_t *start, const uint64_t *chunk_of,
+                                   uint64_t from, uint64_t labels, uint64_t *cbegin, uint32_t *crow,
+                                   unsigned long long *per_block) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += stride) {
+    if (!start[i]) continue;
+    const uint64_t c = chunk_of[i], k = bkey[i];
+    cbegin[c] = i;
+    crow[c] = static_cast<uint32_t>(k >> 32);
+    atomicAdd(per_block + (static_cast<uint32_t>(k) - from) / labels, 1ull);
+  }
+}
+
+// chunk length and sort key (block, length descending); a stable sort keeps row order among equal keys
+__global__ void block_len_kernel(uint64_t chunks, uint64_t count, const uint64_t *bkey, const uint64_t *cbegin,
+                                 uint64_t from, uint64_t labels, uint32_t *clen, uint64_t *ckey, uint64_t *cid) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t c = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; c < chunks; c += stride) {
+    const uint64_t b0 = cbegin[c];
+    const uint32_t len = static_cast<uint32_t>((c + 1 < chunks ? cbegin[c + 1] : count) - b0);
+    const uint64_t b = (static_cast<uint32_t>(bkey[b0]) - from) / labels;
+    clen[c] = len;
+    ckey[c] = (b << 32) | (0xFFFFFFFFu - len);
+    cid[c] = c;
+  }
+}
+
+// one warp per block slice, lane l = chunk l of the slice: its source labels column-major (pad = n), its partial
+__global__ void block_fill_kernel(uint64_t n_slices, const uint32_t *slice_block, const uint64_t *block_slice_first,
+                                  const uint64_t *block_chunk_first, const uint64_t *colbase, const uint64_t *sorted_id,
+                                  const uint64_t *cbegin, const uint32_t *clen, const uint32_t *crow,
+                                  const uint64_t *bkey, const uint64_t *block_ptr, const uint64_t *chunk_of,
+                                  const uint64_t *seg_first, uint32_t pad, uint32_t *idx, uint64_t *slot) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t warps_total = static_cast<uint64_t>(gridDim.x) * (blockDim.x >> 5);
+  for (uint64_t s = static_cast<uint64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); s < n_slices;
+       s += warps_total) {
+    const uint32_t b = slice_block[s];
+    const uint64_t p = block_chunk_first[b] + (s - block_slice_first[b]) * kSliceRows + lane;
+    uint64_t begin = 0, d = ~0ull;
+    uint32_t len = 0;
+    if (p < block_chunk_first[b + 1]) {
+      const uint64_t c = sorted_id[p];
+      const uint64_t r = crow[c];
+      begin = cbegin[c];
+      len = clen[c];
+      d = seg_first[r + 1] - (chunk_of[block_ptr[r + 1]] - c);  // the row's partials end with its block chunks
+    }
+    const uint64_t c0 = colbase[s];
+    const uint32_t width = static_cast<uint32_t>(colbase[s + 1] - c0);
+    uint32_t *dst = idx + c0 * kSliceRows + lane;
+    for (uint32_t k = 0; k < width; ++k)
+      dst[static_cast<size_t>(k) * kSliceRows] = k < len ? static_cast<uint32_t>(bkey[begin + k]) : pad;
+    slot[s * kSliceRows + lane] = d;
   }
 }
 
@@ -551,7 +652,8 @@ void free_graph(Graph &g) {
   if (g.sell_w) cudaFree(g.sell_w);
   if (g.outw_l) cudaFree(g.outw_l);
   void *tile_ptrs[] = {g.seg_slot,  g.tile_base, g.tile_load, g.tile_slice_first, g.tslice_tile,
-                       g.tslice_colbase, g.tile_idx, g.tile_slot, g.tile_work_begin};
+                       g.tslice_colbase, g.tile_idx, g.tile_slot, g.tile_work_begin, g.bslice_colbase, g.block_idx,
+                       g.block_slot};
   for (void *p : tile_ptrs)
     if (p) cudaFree(p);
   void *ptrs[] = {g.label_of,  g.outdeg_l,  g.local_vertex, g.heavy_ptr,    g.heavy_idx, g.seg_row,     g.seg_begin,
@@ -609,6 +711,9 @@ int build_graph(Graph &g, EdgeSource &edges) {
       g.tun.tile_labels = static_cast<uint32_t>(std::min<unsigned long>(kMaxTileLabels, strtoul(s, nullptr, 10))) & ~1u;
     if ((s = getenv("MGB200_TILE_HOT_MB")) != nullptr) g.tun.tile_hot_mb = std::min<uint64_t>(1ull << 20, strtoull(s, nullptr, 10));
     g.tun.tile_chunk = env_u32("MGB200_TILE_CHUNK", g.tun.tile_chunk);
+    if ((s = getenv("MGB200_BLOCK_FROM")) != nullptr) g.tun.block_from = std::min<uint64_t>(strtoull(s, nullptr, 10), ~0u);
+    if ((s = getenv("MGB200_BLOCK_LABELS")) != nullptr) g.tun.block_labels = strtoull(s, nullptr, 10);
+    g.tun.block_chunk = env_u32("MGB200_BLOCK_CHUNK", g.tun.block_chunk);
     if ((s = getenv("MGB200_BARRIER_TIMEOUT_MS")) != nullptr) {
       const unsigned long long ms = strtoull(s, nullptr, 10);
       if (ms) g.tun.barrier_timeout_ms = ms;
@@ -876,7 +981,53 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(cudaMemcpyAsync(row_ptr + g.local_rows, &g.local_edges, sizeof(uint64_t), cudaMemcpyHostToDevice, st));
   }
 
-  // 7. heavy class: tile chunks of the hot sources, CSC + segments of the cold ones
+  // 6b. block class (one partition, unweighted, labels past block_from): the heavy rows' sources >= block_from are
+  // gathered one L2-sized label block at a time (step 9).  Heavy rows come first in key order, so their keys are the
+  // first heavy-edge keys; those >= block_from are compacted (row-major, ascending sources) and cut into chunks of at
+  // most block_chunk edges of one (row, block) run.
+  const uint64_t block_from = g.tun.block_from;
+  const bool block_on = g.part_world == 1 && !g.tun.force_multi_path && !weighted && g.tun.block_labels > 0 &&
+                        n > block_from && n < (1ull << 32) - 1;
+  // at most kMaxBlocks launches per gather: a smaller MGB200_BLOCK_LABELS is raised to that
+  const uint64_t block_labels =
+      block_on ? std::max<uint64_t>(g.tun.block_labels, (n - block_from + kMaxBlocks - 1) / kMaxBlocks) : 0;
+  g.block_labels = block_labels;
+  uint64_t *block_ptr = nullptr, *bkey = nullptr, *bstart = nullptr, *chunk_of = nullptr;
+  if (block_on && g.n_heavy) {
+    const uint64_t nh = g.n_heavy;
+    uint64_t *block_cnt = nullptr, heavy_edges = 0;
+    MGB_CUDA(tmp.alloc(&block_cnt, nh));
+    MGB_CUDA(tmp.alloc(&block_ptr, nh + 1));
+    block_row_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, row_ptr, ekey, block_from, block_cnt);
+    MGB_CUDA(prefix_sum(tmp, block_cnt, block_ptr, nh, st));
+    MGB_CUDA(cudaMemcpyAsync(&g.block_edges, block_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaMemcpyAsync(&heavy_edges, row_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaStreamSynchronize(st));
+    if (g.block_edges) {
+      const uint64_t ne = g.block_edges;
+      MGB_CUDA(tmp.alloc(&bkey, ne));
+      MGB_CUDA(tmp.alloc(&bstart, ne));
+      MGB_CUDA(tmp.alloc(&chunk_of, ne + 1));
+      unsigned long long *d_sel = nullptr;
+      MGB_CUDA(tmp.alloc(&d_sel, 1));
+      size_t bytes = 0;
+      MGB_CUDA(cub::DeviceSelect::If(nullptr, bytes, ekey, bkey, d_sel, static_cast<int64_t>(heavy_edges),
+                                     BlockKey{block_from}, st));
+      void *cub_tmp = nullptr;
+      MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+      MGB_CUDA(cub::DeviceSelect::If(cub_tmp, bytes, ekey, bkey, d_sel, static_cast<int64_t>(heavy_edges),
+                                     BlockKey{block_from}, st));
+      block_start_kernel<<<blocks_for(ne, g.sm_count), kThreads, 0, st>>>(ne, bkey, block_ptr, block_from, block_labels,
+                                                                          g.tun.block_chunk, bstart);
+      MGB_CUDA(prefix_sum(tmp, bstart, chunk_of, ne, st));  // chunk_of[i] = chunk of a starting edge i
+      MGB_CUDA(cudaMemcpyAsync(&g.block_chunks, chunk_of + ne, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+      MGB_CUDA(cudaStreamSynchronize(st));
+      note_mem(g);
+    }
+  }
+  const uint64_t *heavy_block_ptr = g.block_edges ? block_ptr : nullptr;  // block edges per heavy row, if any
+
+  // 7. heavy class: tile chunks of the hot sources, CSC + segments of the cold ones, block chunks of the rest (step 9)
   if (g.n_heavy) {
     const uint64_t nh = g.n_heavy;
     MGB_CUDA(cudaMemcpyAsync(&g.heavy_edges, row_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -884,7 +1035,9 @@ int build_graph(Graph &g, EdgeSource &edges) {
     // 7a. tiles: every owner's hot prefix cut into T-label windows; a window starts on an even label (16-byte aligned)
     const uint32_t T = weighted ? 0u : g.tun.tile_labels;
     const uint32_t owners = (g.part_world > 1 && !map.global_order) ? g.part_world : 1u;
-    const TileSet tiles{Dealer{n, owners}, (g.tun.tile_hot_mb << 20) / sizeof(double) / owners};
+    uint64_t tile_hot = T ? (g.tun.tile_hot_mb << 20) / sizeof(double) / owners : 0;
+    if (block_on) tile_hot = std::min(tile_hot, block_from);  // sources past block_from belong to the block class
+    const TileSet tiles{Dealer{n, owners}, tile_hot};
     std::vector<uint32_t> t_lo, t_hi, t_base, t_load;
     for (uint32_t q = 0; T && q < owners; ++q) {
       const uint64_t s0 = tiles.owners.start(q), end = s0 + std::min(tiles.hot, tiles.owners.count(q));
@@ -928,14 +1081,14 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(tmp.alloc(&row_cold_segs, nh));
     MGB_CUDA(tmp.alloc(&cold_seg_first, nh + 1));
     tile_row_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, nt, indeg_local, pair_cnt, pair_chunks,
-                                                                    cold_deg, row_chunks);
+                                                                    heavy_block_ptr, cold_deg, row_chunks);
     MGB_CUDA(keep_alloc(g, &g.heavy_ptr, nh + 1));
     MGB_CUDA(prefix_sum(tmp, cold_deg, g.heavy_ptr, nh, st));
     uint64_t cold_edges = 0;
     MGB_CUDA(cudaMemcpyAsync(&cold_edges, g.heavy_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     if (nt) MGB_CUDA(cudaMemcpyAsync(&g.tile_chunks, pair_chunk_first + pairs, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
-    g.tiled_edges = g.heavy_edges - cold_edges;
+    g.tiled_edges = g.heavy_edges - cold_edges - g.block_edges;
     if (!getenv("MGB200_SEGMENT_EDGES")) {
       // one warp per segment: aim for >= 8 segments per resident warp (64 warps/SM) so the tail is short
       // when a partition holds few cold heavy edges (multi-GPU, or most of them tiled), capped at 4096 edges
@@ -944,25 +1097,25 @@ int build_graph(Graph &g, EdgeSource &edges) {
       seg = (seg / 256) * 256;
       g.segment_edges = static_cast<uint32_t>(std::min<uint64_t>(4096, std::max<uint64_t>(256, seg)));
     }
-    seg_count_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, cold_deg, row_chunks, g.segment_edges,
-                                                                     row_parts, row_cold_segs);
+    seg_count_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, cold_deg, row_chunks, heavy_block_ptr, chunk_of,
+                                                                     g.segment_edges, row_parts, row_cold_segs);
     MGB_CUDA(keep_alloc(g, &g.seg_first, nh + 1));
     MGB_CUDA(prefix_sum(tmp, row_parts, g.seg_first, nh, st));
     MGB_CUDA(prefix_sum(tmp, row_cold_segs, cold_seg_first, nh, st));
     MGB_CUDA(cudaMemcpyAsync(&g.n_seg, g.seg_first + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaMemcpyAsync(&g.n_cold_seg, cold_seg_first + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-    // 7b. cold edges: the heavy rows' keys without the tiled ones (order kept), as CSC + fixed-size segments
+    // 7b. cold edges: the heavy rows' keys without the tiled and block ones (order kept), as CSC + fixed-size segments
     const uint64_t *cold_keys = ekey;
-    if (g.tiled_edges) {
+    if (g.tiled_edges || g.block_edges) {
       unsigned long long *d_sel = nullptr;
       MGB_CUDA(tmp.alloc(&d_sel, 1));
       size_t bytes = 0;
       MGB_CUDA(cub::DeviceSelect::If(nullptr, bytes, ekey, ekey_alt, d_sel, static_cast<int64_t>(g.heavy_edges),
-                                     ColdKey{tiles}, st));
+                                     ColdKey{tiles, block_on ? block_from : n + 1}, st));
       void *cub_tmp = nullptr;
       MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
       MGB_CUDA(cub::DeviceSelect::If(cub_tmp, bytes, ekey, ekey_alt, d_sel, static_cast<int64_t>(g.heavy_edges),
-                                     ColdKey{tiles}, st));
+                                     ColdKey{tiles, block_on ? block_from : n + 1}, st));
       cold_keys = ekey_alt;
     }
     MGB_CUDA(keep_alloc(g, &g.heavy_idx, cold_edges));
@@ -975,11 +1128,12 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(cudaStreamSynchronize(st));
     MGB_CUDA(keep_alloc(g, &g.seg_row, g.n_cold_seg));
     MGB_CUDA(keep_alloc(g, &g.seg_begin, g.n_cold_seg));
-    if (g.tile_chunks) MGB_CUDA(keep_alloc(g, &g.seg_slot, g.n_cold_seg));
+    if (g.tile_chunks || g.block_chunks) MGB_CUDA(keep_alloc(g, &g.seg_slot, g.n_cold_seg));
     MGB_CUDA(keep_alloc(g, &g.seg_partial, g.n_seg));
     MGB_CUDA(keep_alloc(g, &g.heavy_sums, nh));
     segment_fill_kernel<<<blocks_for(nh * 32, g.sm_count), kThreads, 0, st>>>(
-        nh, g.heavy_ptr, cold_seg_first, g.segment_edges, g.seg_first, g.seg_row, g.seg_begin, g.seg_slot);
+        nh, g.heavy_ptr, cold_seg_first, g.segment_edges, g.seg_first, heavy_block_ptr, chunk_of, g.seg_row, g.seg_begin,
+        g.seg_slot);
     // 7c. tile chunks -> per tile, SELL-32 slices of chunks sorted by length (ties: row order)
     if (g.tile_chunks) {
       std::vector<unsigned long long> per_tile(nt);
@@ -1098,6 +1252,79 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(keep_alloc(g, &g.sell_work_items, g.sell_work));
     work_item_kernel<<<(g.sell_work + kThreads - 1) / kThreads, kThreads, 0, st>>>(g.sell_work, g.sell_work_begin,
                                                                                   g.sell_colbase, g.sell_work_items);
+  }
+
+  // 9. block chunks -> per block, SELL-32 slices of chunks sorted by length (ties: row order); empty blocks are skipped
+  if (g.block_chunks) {
+    const uint64_t nb = (n - block_from + block_labels - 1) / block_labels, nc = g.block_chunks, ne = g.block_edges;
+    uint64_t *cbegin = nullptr, *ckey = nullptr, *ckey_alt = nullptr, *cid = nullptr, *cid_alt = nullptr;
+    uint32_t *crow = nullptr, *clen = nullptr;
+    unsigned long long *per_block = nullptr;
+    MGB_CUDA(tmp.alloc(&cbegin, nc));
+    MGB_CUDA(tmp.alloc(&ckey, nc));
+    MGB_CUDA(tmp.alloc(&ckey_alt, nc));
+    MGB_CUDA(tmp.alloc(&cid, nc));
+    MGB_CUDA(tmp.alloc(&cid_alt, nc));
+    MGB_CUDA(tmp.alloc(&crow, nc));
+    MGB_CUDA(tmp.alloc(&clen, nc));
+    MGB_CUDA(tmp.alloc(&per_block, nb));
+    MGB_CUDA(cudaMemsetAsync(per_block, 0, nb * sizeof(unsigned long long), st));
+    block_chunk_kernel<<<blocks_for(ne, g.sm_count), kThreads, 0, st>>>(ne, bkey, bstart, chunk_of, block_from,
+                                                                        block_labels, cbegin, crow, per_block);
+    block_len_kernel<<<blocks_for(nc, g.sm_count), kThreads, 0, st>>>(nc, ne, bkey, cbegin, block_from, block_labels,
+                                                                      clen, ckey, cid);
+    std::vector<unsigned long long> counts_b(nb);
+    MGB_CUDA(cudaMemcpyAsync(counts_b.data(), per_block, nb * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaStreamSynchronize(st));
+    std::vector<uint64_t> chunk_first(nb + 1, 0), slice_first(nb + 1, 0);
+    std::vector<uint32_t> slice_block;
+    g.block_slice_first.assign(1, 0);
+    g.block_lo.clear();
+    for (uint64_t b = 0; b < nb; ++b) {
+      chunk_first[b + 1] = chunk_first[b] + counts_b[b];
+      const uint64_t slices = (counts_b[b] + kSliceRows - 1) / kSliceRows;
+      slice_first[b + 1] = slice_first[b] + slices;
+      slice_block.insert(slice_block.end(), slices, static_cast<uint32_t>(b));
+      if (slices) {
+        g.block_slice_first.push_back(slice_first[b + 1]);
+        g.block_lo.push_back(static_cast<uint32_t>(block_from + b * block_labels));
+      }
+    }
+    const uint64_t ns = slice_first[nb];
+    g.block_slices = ns;
+    uint64_t *d_chunk_first = nullptr, *d_slice_first = nullptr;
+    uint32_t *d_slice_block = nullptr;
+    MGB_CUDA(tmp.alloc(&d_chunk_first, nb + 1));
+    MGB_CUDA(tmp.alloc(&d_slice_first, nb + 1));
+    MGB_CUDA(tmp.alloc(&d_slice_block, ns));
+    MGB_CUDA(cudaMemcpyAsync(d_chunk_first, chunk_first.data(), (nb + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    MGB_CUDA(cudaMemcpyAsync(d_slice_first, slice_first.data(), (nb + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    MGB_CUDA(cudaMemcpyAsync(d_slice_block, slice_block.data(), ns * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    const uint64_t *sorted_id = nullptr;
+    {  // stable: equal (block, length) keep row order, so the layout is a function of the graph alone
+      cub::DoubleBuffer<uint64_t> kb(ckey, ckey_alt);
+      cub::DoubleBuffer<uint64_t> vb(cid, cid_alt);
+      size_t bytes = 0;
+      MGB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, kb, vb, nc, 0, 32 + bits_for(nb), st));
+      void *cub_tmp = nullptr;
+      MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+      MGB_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp, bytes, kb, vb, nc, 0, 32 + bits_for(nb), st));
+      sorted_id = vb.Current();
+    }
+    uint64_t *width = nullptr;
+    MGB_CUDA(tmp.alloc(&width, ns));
+    tile_width_kernel<<<blocks_for(ns, g.sm_count), kThreads, 0, st>>>(ns, d_slice_block, d_slice_first, d_chunk_first,
+                                                                      sorted_id, clen, width);
+    MGB_CUDA(keep_alloc(g, &g.bslice_colbase, ns + 1));
+    MGB_CUDA(prefix_sum(tmp, width, g.bslice_colbase, ns, st));
+    uint64_t total_cols = 0;
+    MGB_CUDA(cudaMemcpyAsync(&total_cols, g.bslice_colbase + ns, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaStreamSynchronize(st));
+    MGB_CUDA(keep_alloc(g, &g.block_idx, total_cols * kSliceRows));
+    MGB_CUDA(keep_alloc(g, &g.block_slot, ns * kSliceRows));
+    block_fill_kernel<<<blocks_for(ns * 32, g.sm_count), kThreads, 0, st>>>(
+        ns, d_slice_block, d_slice_first, d_chunk_first, g.bslice_colbase, sorted_id, cbegin, clen, crow, bkey, block_ptr,
+        chunk_of, g.seg_first, static_cast<uint32_t>(n), g.block_idx, g.block_slot);
   }
   note_mem(g);
   MGB_CUDA(cudaGetLastError());

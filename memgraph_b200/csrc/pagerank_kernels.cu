@@ -670,6 +670,60 @@ __global__ void __launch_bounds__(kTileThreads, 2) heavy_tiles_kernel(const Tile
   }
 }
 
+// Block passes (graph_build.cu step 9): the heavy rows' in-edges from labels >= block_from, one label block per launch,
+// so the block's part of contrib is read from HBM about once per pass instead of costing a sector per gather.  One warp
+// per slice, one lane per chunk: the lane adds its chunk in ascending source order and stores the chunk's partial (no
+// atomics, the same bits every run).
+struct BlockArgs {
+  const uint32_t *idx;      // [32 * columns] source labels, column-major per slice, pad = n
+  const uint64_t *colbase;  // [slices + 1]
+  const uint64_t *slot;     // [32 * slices] partial of each lane's chunk, ~0 = padding lane
+  uint64_t slice_begin, slice_end;
+  const double *block;      // contrib_in + first label of the block
+  uint32_t block_bytes;      // evict_last span
+  uint32_t tail_bytes;       // block .. the end of the vector (padding slot included): evict_first past the block
+  const double *contrib_in;
+  double *seg_partial;
+  IterState *state;
+};
+__global__ void __launch_bounds__(kBlockThreads) cold_block_kernel(const BlockArgs a) {
+  if (ld_volatile_int(&a.state->done)) return;
+  const int lane = threadIdx.x & 31;
+  const uint64_t warps_total = static_cast<uint64_t>(gridDim.x) * kWarpsPerBlock;
+  const uint64_t pol = make_evict_first_policy();
+  uint64_t gpol;  // evict_last over the block, evict_first past it (the padding slot); DESIGN.md §4: beats default priority
+  asm volatile("createpolicy.range.global.L2::evict_last.L2::evict_first.b64 %0, [%1], %2, %3;"
+               : "=l"(gpol)
+               : "l"(a.block), "r"(a.block_bytes), "r"(a.tail_bytes));
+  for (uint64_t s = a.slice_begin + static_cast<uint64_t>(blockIdx.x) * kWarpsPerBlock + (threadIdx.x >> 5);
+       s < a.slice_end; s += warps_total) {
+    const uint64_t c0 = a.colbase[s], ncols = a.colbase[s + 1] - c0;
+    const uint64_t slot = a.slot[s * kSliceRows + lane];
+    const uint32_t *p = a.idx + c0 * kSliceRows + lane;
+    double acc = 0.0;
+    uint32_t nxt[kUnroll];
+#pragma unroll
+    for (int j = 0; j < kUnroll; ++j)
+      if (static_cast<uint64_t>(j) < ncols) nxt[j] = ld_index(p + static_cast<size_t>(j) * kSliceRows, pol);
+    for (uint64_t k = 0; k < ncols; k += kUnroll) {
+      uint32_t src[kUnroll];
+      double v[kUnroll];
+#pragma unroll
+      for (int j = 0; j < kUnroll; ++j) src[j] = nxt[j];
+#pragma unroll
+      for (int j = 0; j < kUnroll; ++j)  // the next batch of labels travels while this batch is gathered
+        if (k + kUnroll + j < ncols) nxt[j] = ld_index(p + static_cast<size_t>(k + kUnroll + j) * kSliceRows, pol);
+#pragma unroll
+      for (int j = 0; j < kUnroll; ++j)
+        if (k + j < ncols) v[j] = ld_contrib(a.contrib_in + src[j], gpol);
+#pragma unroll
+      for (int j = 0; j < kUnroll; ++j)
+        if (k + j < ncols) acc += v[j];  // ascending source order inside the chunk
+    }
+    if (slot != ~0ull) a.seg_partial[slot] = acc;
+  }
+}
+
 struct HeavyArgs {
   const uint64_t *heavy_ptr;
   const uint32_t *heavy_idx;
@@ -1125,12 +1179,41 @@ int launch_sell_stream(Graph &g, const SellArgs &s) {
   return MGB200_OK;
 }
 
+// The block passes over `vec`, one launch per non-empty block, in block order on the main stream
+int launch_block_passes(Graph &g, const double *vec, uint64_t *launches) {
+  const uint64_t grid_cap = static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(cold_block_kernel)));
+  for (size_t b = 0; b + 1 < g.block_slice_first.size(); ++b) {
+    BlockArgs a{};
+    a.idx = g.block_idx;
+    a.colbase = g.bslice_colbase;
+    a.slot = g.block_slot;
+    a.slice_begin = g.block_slice_first[b];
+    a.slice_end = g.block_slice_first[b + 1];
+    a.block = vec + g.block_lo[b];
+    const uint64_t tail = std::min<uint64_t>((g.n + 1 - g.block_lo[b]) * sizeof(double), 0xFFFFFF00ull);
+    a.block_bytes = static_cast<uint32_t>(std::min<uint64_t>(g.block_labels * sizeof(double), tail));
+    a.tail_bytes = static_cast<uint32_t>(tail);
+    a.contrib_in = vec;
+    a.seg_partial = g.seg_partial;
+    a.state = g.state;
+    const int grid = static_cast<int>(std::min(grid_cap, ceil_div(a.slice_end - a.slice_begin, kWarpsPerBlock)));
+    cold_block_kernel<<<grid, kBlockThreads, 0, g.stream>>>(a);
+    MGB_CUDA(cudaGetLastError());
+    ++*launches;
+  }
+  return MGB200_OK;
+}
+
 // Heavy-row partials: the tile chunks (shared-memory reads, a 2-byte offset stream; one CTA per work item, one per SM,
 // as a tile takes most of the SM's shared memory) and the cold segments (random HBM gathers) write disjoint partials
 // and wait on different units, so with both present the cold segments run on a stream of their own next to the tile
 // kernel, joined back before the caller's row sums.  The tile kernel goes first: its CTAs need half an SM each and
 // would wait behind a full grid of segment CTAs.  The segment grid leaves `reserve_ctas` CTA slots to other kernels.
 int launch_heavy_partials(Graph &g, const HeavyArgs &h, uint64_t reserve_ctas, uint64_t *launches) {
+  // the block passes first, on the main stream: they write partials of their own, and next to the SELL epilogue they
+  // measured faster than between the SELL rows and its fork (DESIGN.md §4)
+  const int rc = launch_block_passes(g, h.contrib_in, launches);
+  if (rc) return rc;
   void (*const seg_fn)(HeavyArgs) = h.heavy_w != nullptr           ? heavy_segments_kernel<kPathRange, true>
                                     : h.window.path == kPathFlags  ? heavy_segments_kernel<kPathFlags>
                                     : h.window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
@@ -1196,7 +1279,8 @@ int launch_barrier(Graph &g) {
   return MGB200_OK;
 }
 
-// One iteration.  Main stream: (iteration 1: zero-row contribution refresh) -> SELL rows -> heavy segments ->
+// One iteration.  Main stream: (iteration 1: zero-row contribution refresh) -> SELL rows -> heavy partials (block
+// passes, tiles, segments; all inside the heavy_segments event class) ->
 // heavy finish -> [join] -> iteration end.  Side stream: the SELL epilogue, forked after the SELL rows:
 // it is the kernel that pushes contributions to the peer GPUs (NVLink-bound), so it overlaps with the
 // heavy-row kernels (L2-gather-bound) instead of queueing behind them.  Every kernel returns immediately
@@ -1315,7 +1399,7 @@ int launch_gather_phase(Graph &g, const double *vec_in, uint64_t *launch_count, 
     ++launches;
   }
   if (g.n_seg > 0) {
-    const HeavyArgs h = make_heavy_args(g, vec_in, window, weighted);  // weighted graphs have no tile class
+    const HeavyArgs h = make_heavy_args(g, vec_in, window, weighted);  // weighted graphs have no tile or block class
     int rc = launch_heavy_partials(g, h, 0, &launches);
     if (rc) return rc;
     if (heavy_row_sums) {

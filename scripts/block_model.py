@@ -1,0 +1,67 @@
+"""Counting model of the block class (graph_build.cu steps 6b and 9, one partition): which in-edges of the heavy rows
+come from a source label >= --block-from, how many (row, label block) chunks of at most --block-chunk edges they make,
+in how many non-empty blocks, and how long the chunks are.
+
+It relabels like the build (in-degree descending, out-degree descending, id ascending), so its counts equal the
+`block_edges`, `block_chunks` and `blocks` of PageRankGraph.info for the same edges and knobs
+(tests/test_gpu_block_gather.py).
+
+    python scripts/block_model.py --scale 22 [--block-from 2097152 --block-labels 2097152 --block-chunk 16 --heavy-min 1024]
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+
+def block_model(n, frm, to, block_from=2 << 20, block_labels=2 << 20, block_chunk=16, heavy_min=1024, max_blocks=4096):
+    frm = np.asarray(frm, dtype=np.int64)
+    to = np.asarray(to, dtype=np.int64)
+    indeg = np.bincount(to, minlength=n)
+    outdeg = np.bincount(frm, minlength=n)
+    order = np.lexsort((np.arange(n), -outdeg, -indeg))  # sorted position -> vertex
+    label = np.empty(n, dtype=np.int64)
+    label[order] = np.arange(n)
+    n_heavy = int(np.count_nonzero(indeg >= heavy_min))
+    src, dst = label[frm], label[to]
+    out = {"n": n, "m": len(frm), "heavy_rows": n_heavy, "heavy_edges": int(np.count_nonzero(dst < n_heavy)),
+           "block_edges": 0, "block_chunks": 0, "blocks": 0, "chunk_length_histogram": {}}
+    if block_labels == 0 or n <= block_from:
+        return out
+    labels = max(block_labels, -(-(n - block_from) // max_blocks))  # the build keeps <= max_blocks blocks
+    cold = (dst < n_heavy) & (src >= block_from)
+    nb = -(-(n - block_from) // labels)
+    pair, cnt = np.unique(dst[cold] * nb + (src[cold] - block_from) // labels, return_counts=True)
+    lengths = np.concatenate([np.repeat(block_chunk, int((cnt // block_chunk).sum())), (cnt % block_chunk)[cnt % block_chunk > 0]])
+    edges = [1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1 << 62]
+    hist, _ = np.histogram(lengths, bins=edges)
+    out["block_edges"] = int(cold.sum())
+    out["block_chunks"] = int((-(-cnt // block_chunk)).sum())
+    out["blocks"] = int(len(np.unique(pair % nb)))
+    out["chunk_length_histogram"] = {f"[{lo},{hi})" if hi < 1 << 62 else f">={lo}": int(h)
+                                     for lo, hi, h in zip(edges[:-1], edges[1:], hist)}
+    out["edges_per_chunk"] = out["block_edges"] / max(out["block_chunks"], 1)
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--scale", type=int, default=20)
+    ap.add_argument("--edge-factor", type=int, default=16)
+    ap.add_argument("--seed", type=int, default=42)
+    ap.add_argument("--block-from", type=int, default=2 << 20)
+    ap.add_argument("--block-labels", type=int, default=2 << 20)
+    ap.add_argument("--block-chunk", type=int, default=16)
+    ap.add_argument("--heavy-min", type=int, default=1024)
+    args = ap.parse_args()
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    import memgraph_b200 as mg
+    n, m = 1 << args.scale, args.edge_factor << args.scale
+    f, t = mg.rmat_edges_host(args.scale, m, seed=args.seed)
+    print(json.dumps(block_model(n, f, t, args.block_from, args.block_labels, args.block_chunk, args.heavy_min)))
+
+
+if __name__ == "__main__":
+    main()
