@@ -88,6 +88,30 @@ int mgb200_bc_run(mgb200_bfs_graph *g, int directed, uint64_t source_begin, uint
 int mgb200_betweenness_centrality(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to, int directed,
                                   int normalized, double *bc_out);
 
+/*
+ * Weakly connected components on the same device graph: the result of the reference's weakly_connected_components.get
+ * (mage/cpp/connectivity_module/connectivity_module.cpp:41-84), a BFS over the undirected view (out- and in-lists
+ * together) from every unvisited vertex in dense order.  component_out[v] is the number of v's component; components
+ * are numbered in the order of their smallest vertex id.  Self-loops and multi-edges change nothing.  The work is
+ * integer union-find whose roots are the components' smallest ids, so two runs are byte-identical.  Without a device
+ * every call fails with MGB200_ERR_CUDA.
+ */
+typedef struct mgb200_wcc_stats {
+  uint64_t components;         /* number of components                                    */
+  uint64_t largest_component;  /* vertices in the largest one                             */
+  uint64_t skipped_vertices;   /* vertices whose remaining lists the finish phase skipped */
+  uint64_t edges_inspected;    /* adjacency entries read, sampling and finish together    */
+  double run_ms;               /* CUDA-event time, parent init .. last label written      */
+  uint64_t kernel_launches;
+} mgb200_wcc_stats;
+
+/* component_out: n int64 values in host memory.  n == 0 returns MGB200_OK with zero components. */
+int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats *stats);
+
+/* The reference procedure's arithmetic end to end, on device 0: host COO (uint64 endpoints < n) -> component_out[n]. */
+int mgb200_weakly_connected_components(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to,
+                                       int64_t *component_out);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -37,6 +37,11 @@ class BcStats(ctypes.Structure):
                 ("run_ms", f64), ("kernel_launches", u64)]
 
 
+class WccStats(ctypes.Structure):
+    _fields_ = [("components", u64), ("largest_component", u64), ("skipped_vertices", u64), ("edges_inspected", u64),
+                ("run_ms", f64), ("kernel_launches", u64)]
+
+
 class KatzStats(ctypes.Structure):
     _fields_ = [("iterations", u64), ("max_out_degree", u64), ("gamma", f64), ("iterate_ms", f64),
                 ("kernel_launches", u64), ("tie_order_runs", u64)]
@@ -90,6 +95,8 @@ EXPORTS = {
     "mgb200_bfs_run": (i32, [vp, u64, i32, ctypes.c_int64, ctypes.c_int64, vp, i32, ctypes.POINTER(BfsStats)]),
     "mgb200_bc_run": (i32, [vp, i32, u64, u64, ABORT_FN, vp, vp, i32, ctypes.POINTER(BcStats)]),
     "mgb200_betweenness_centrality": (i32, [u64, u64, vp, vp, i32, i32, vp]),
+    "mgb200_wcc_run": (i32, [vp, vp, ctypes.POINTER(WccStats)]),
+    "mgb200_weakly_connected_components": (i32, [u64, u64, vp, vp, vp]),
     # include/mgb200_katz.h
     "mgb200_katz_run": (i32, [vp, f64, f64, u64, vp, ctypes.POINTER(KatzStats)]),
     "mgb200_katz_centrality": (i32, [u64, u64, vp, vp, f64, f64, u64, vp, ctypes.POINTER(u64)]),

@@ -4,7 +4,7 @@
     memgraph_b200/_build/pagerank.so             drop-in Memgraph query module (mgp_init_module / mgp_shutdown_module)
     memgraph_b200/_build/libmgp_fake_host.so     fake mgp host used by the tests to load query modules without Memgraph
     memgraph_b200/_build/<module>.so             the other query modules (gpu_bfs, katz_centrality, betweenness_centrality,
-                                                 cugraph.*), same linking as pagerank.so
+                                                 weakly_connected_components, cugraph.*), same linking as pagerank.so
 
 Objects are rebuilt only when a source or header is newer.  `python -m memgraph_b200.build` builds everything.
 """
@@ -30,7 +30,8 @@ NVCC_FLAGS = [
     "-I", INCLUDE, "-I", CSRC,
     "-diag-suppress", "1444",  # cub::TransformInputIterator deprecation notice
 ]
-CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu"]
+CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu",
+                "wcc.cu"]
 HEADERS = [os.path.join(CSRC, "core.hpp"), os.path.join(CSRC, "bfs_graph.hpp"), os.path.join(CSRC, "rmat.hpp"), os.path.join(CSRC, "sell_stream.cuh"),
            os.path.join(INCLUDE, "mgb200_pagerank.h"), os.path.join(INCLUDE, "mgb200_bfs.h"),
            os.path.join(INCLUDE, "mgb200_katz.h"), os.path.join(INCLUDE, "mgb200_personalized.h"), os.path.join(CSRC, "katz_heap.hpp"),
@@ -43,6 +44,8 @@ BC_HOST_LIB = os.path.join(OUT, "libmgp_bc_host.so")
 BFS_MODULE_LIB = os.path.join(OUT, "gpu_bfs.so")
 KATZ_MODULE_LIB = os.path.join(OUT, "katz_centrality.so")
 BC_MODULE_LIB = os.path.join(OUT, "betweenness_centrality.so")
+WCC_MODULE_LIB = os.path.join(OUT, "weakly_connected_components.so")
+WCC_HOST_LIB = os.path.join(OUT, "libmgp_wcc_host.so")
 
 
 def _newer(target, deps):
@@ -129,6 +132,18 @@ def build_bc_module(objs, verbose=False):
         _run([NVCC, "-shared", "-cudart", "static", "-o", BC_MODULE_LIB, obj] + objs)
 
 
+def build_wcc_module(objs, verbose=False):
+    """weakly_connected_components.so: weakly connected components behind the reference module's name and signature."""
+    src = os.path.join(CSRC, "weakly_connected_components_module.cpp")
+    obj = os.path.join(OUT, "weakly_connected_components_module.o")
+    if _newer(obj, [src] + HEADERS):
+        if verbose:
+            print("g++ weakly_connected_components_module.cpp", flush=True)
+        _run([CXX, "-std=c++20", "-O2", "-fPIC", "-fvisibility=hidden", "-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj])
+    if _newer(WCC_MODULE_LIB, objs + [obj]):
+        _run([NVCC, "-shared", "-cudart", "static", "-o", WCC_MODULE_LIB, obj] + objs)
+
+
 CUGRAPH_MODULE_LIBS = {0: os.path.join(OUT, "cugraph.pagerank.so"), 1: os.path.join(OUT, "cugraph.personalized_pagerank.so")}
 
 
@@ -169,6 +184,16 @@ def build_bc_host(verbose=False):
         _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", BC_HOST_LIB, BC_HOST_SRC, "-ldl"])
 
 
+WCC_HOST_SRC = os.path.join(REPO, "tests", "mgp_wcc_host.cpp")  # the BOOLEAN host plus an INTEGER-column call
+
+
+def build_wcc_host(verbose=False):
+    if _newer(WCC_HOST_LIB, [WCC_HOST_SRC, BC_HOST_SRC, FAKE_HOST_SRC] + HEADERS):
+        if verbose:
+            print("g++ mgp_wcc_host.cpp", flush=True)
+        _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", WCC_HOST_LIB, WCC_HOST_SRC, "-ldl"])
+
+
 def build_all(verbose=False):
     objs = build_core(verbose)
     if os.path.exists(os.path.join(CSRC, "pagerank_module.cpp")):
@@ -188,6 +213,9 @@ def build_all(verbose=False):
     if os.path.exists(os.path.join(CSRC, "betweenness_centrality_module.cpp")):
         build_bc_module(objs, verbose)
         out["betweenness_centrality_module"] = BC_MODULE_LIB
+    if os.path.exists(os.path.join(CSRC, "weakly_connected_components_module.cpp")):
+        build_wcc_module(objs, verbose)
+        out["weakly_connected_components_module"] = WCC_MODULE_LIB
     if os.path.exists(os.path.join(CSRC, "gpu_bfs_module.cpp")):
         out["bfs_module"] = BFS_MODULE_LIB
     if os.path.exists(os.path.join(CSRC, "pagerank_module.cpp")):
@@ -197,6 +225,9 @@ def build_all(verbose=False):
     if os.path.exists(BC_HOST_SRC):
         build_bc_host(verbose)
         out["bc_host"] = BC_HOST_LIB
+    if os.path.exists(WCC_HOST_SRC):
+        build_wcc_host(verbose)
+        out["wcc_host"] = WCC_HOST_LIB
     return out
 
 

@@ -1,6 +1,6 @@
 // memgraph_b200/csrc/bfs_graph.hpp -- the device graph behind the opaque mgb200_bfs_graph handle (include/mgb200_bfs.h).
-// Shared by the breadth-first expansion (bfs.cu), which builds it, and betweenness centrality (betweenness.cu),
-// which walks the same CSR + CSC.
+// Shared by the breadth-first expansion (bfs.cu), which builds it, betweenness centrality (betweenness.cu) and weakly
+// connected components (wcc.cu), which walk the same CSR + CSC.
 #pragma once
 
 #include <cuda_runtime.h>
