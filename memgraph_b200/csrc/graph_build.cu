@@ -204,7 +204,11 @@ struct IndexFlags {
     }
     const uint32_t local = label - s0;
     if (local < table_per_owner) return kIdxL1Hot | (owner * table_per_owner + local);
-    return label | (local < l2_hot ? kIdxL2Hot : 0u) | (l1_hot != kNoL1Hints && local < l1_hot ? kIdxL1Hot : 0u);
+    const bool l2 = local < l2_hot;
+    // with a table, code 01 means "table slot", so a label outside the L2 window (L2_HOT_MB=0, or an L1 window larger
+    // than the L2 one) keeps no L1 flag: L1-hot without L2-hot would read as a slot
+    const bool l1 = l1_hot != kNoL1Hints && local < l1_hot && (l2 || table_per_owner == 0);
+    return label | (l2 ? kIdxL2Hot : 0u) | (l1 ? kIdxL1Hot : 0u);
   }
 };
 
@@ -718,6 +722,10 @@ int build_graph(Graph &g, EdgeSource &edges) {
       const unsigned long long ms = strtoull(s, nullptr, 10);
       if (ms) g.tun.barrier_timeout_ms = ms;
     }
+  }
+  if (edges.weighted()) {  // weighted gathers exist on the range path only: the knobs that leave it do not apply
+    g.tun.idx_flags = 0;
+    g.tun.force_multi_path = false;
   }
   for (auto &e : g.ev) MGB_CUDA(cudaEventCreate(&e));
   cudaStream_t st = g.stream;

@@ -102,7 +102,9 @@ struct GatherPolicy {
 __device__ __forceinline__ GatherPolicy make_gather_policy(const double *contrib_in, const GatherWindow &w) {
   GatherPolicy p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p.cold));
-  if (w.path == kPathRange) {  // single partition, or partition-unaware legacy mode: one range policy over the prefix
+  if (w.path == kPathRange && w.hot_bytes == 0) {  // MGB200_L2_HOT_MB=0: every gather evict_first, and no
+    p.hot = p.cold;  // createpolicy.range with a zero primary size (a case the PTX ISA does not describe)
+  } else if (w.path == kPathRange) {  // single partition, or partition-unaware legacy mode: one range policy over the prefix
     asm volatile("createpolicy.range.global.L2::evict_last.L2::evict_first.b64 %0, [%1], %2, %3;"
                  : "=l"(p.hot)
                  : "l"(contrib_in), "r"(w.hot_bytes), "r"(w.total_bytes));

@@ -115,6 +115,31 @@ def test_weight_property_isolated_vertices_and_seeds():
     assert fh.host().fh_live_objects() == 0
 
 
+@pytest.mark.gpu
+@needs_modules
+@pytest.mark.parametrize("env", [{"MGB200_IDX_FLAGS": "1"}, {"MGB200_FORCE_MULTI_PATH": "1"}])
+def test_weight_property_under_gather_path_knobs(env, monkeypatch):
+    """The gather-path knobs are tuning only: a weighted graph stays on the one gather path that has weights."""
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    rng = np.random.default_rng(13)
+    n, m = 3000, 40000
+    gids = (np.arange(n) * 3 + 11).tolist()
+    s, d = rng.integers(0, n, m), rng.integers(0, n, m)
+    src, dst = [gids[i] for i in s], [gids[i] for i in d]
+    w = rng.uniform(0.1, 4.0, m)
+    used = sorted(set(src) | set(dst))
+    dense = {g: i for i, g in enumerate(used)}
+    f, t = [dense[x] for x in src], [dense[x] for x in dst]
+    with fh.Module(fh.CUGRAPH_PAGERANK_SO) as m1, fh.Graph(gids, src, dst) as g:
+        g.set_edge_property("weight", src, w)
+        nodes, ranks = m1.call(g, 100, 0.85, 1e-10)
+    ref, _, _ = oracle_cugraph_pagerank(len(used), f, t, weights=w, epsilon=1e-10)
+    assert nodes.tolist() == used
+    assert float(np.max(np.abs(ranks - ref) / ref)) < 1e-9
+    assert fh.host().fh_live_objects() == 0
+
+
 @needs_modules
 @pytest.mark.parametrize("path", [fh.CUGRAPH_PAGERANK_SO, fh.CUGRAPH_PERSONALIZED_SO, fh.BFS_MODULE_SO])
 def test_modules_import_only_declared_mgp_symbols_and_no_cuda(path):

@@ -20,8 +20,12 @@ def _device_count():
         return 0
 
 
-def run_partitioned(mg, n, f, t, world, **kw):
-    graphs = [mg.PageRankGraph.from_arrays(n, f, t, device=q, part_rank=q, part_world=world) for q in range(world)]
+def run_partitioned(mg, n, f, t, world, devices=None, **kw):
+    """Partition q on device devices[q] (default: device q), one host thread each; -> (ranks by vertex, per-partition
+    (ranks, vertices, RunStats), per-partition info)."""
+    devices = list(range(world)) if devices is None else devices
+    graphs = [mg.PageRankGraph.from_arrays(n, f, t, device=devices[q], part_rank=q, part_world=world)
+              for q in range(world)]
     for g in graphs:
         g.connect_peers(local_graphs=graphs)
     results = [None] * world
