@@ -112,6 +112,36 @@ int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats
 int mgb200_weakly_connected_components(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to,
                                        int64_t *component_out);
 
+/*
+ * Bridges and biconnected components of the undirected multigraph view (every edge in both endpoints' lists), the
+ * partition of the reference's bridges.get and biconnected_components.get (mage/cpp/bridges_module,
+ * mage/cpp/biconnected_components_module).  Tarjan-Vishkin on a breadth-first spanning forest rooted at each
+ * component's smallest id; all integer work, so two runs are byte-identical.  Per edge e of the COO the graph was built
+ * from, in the same order:
+ *   bridge_out[e] = 1 iff removing e disconnects its endpoints (a doubled edge is never a bridge, a self-loop never is);
+ *   bcc_out[e]    = the number of e's biconnected component, -1 for a self-loop.  Components are numbered in the order
+ *                   of their first edge in the COO, so the numbering depends neither on thread order nor on the tree.
+ * Without a device every call fails with MGB200_ERR_CUDA.
+ */
+typedef struct mgb200_biconnectivity_stats {
+  uint64_t trees;            /* spanning trees with at least one edge                              */
+  uint32_t forest_depth;     /* deepest BFS level of the forest (0 when no vertex has a parent)    */
+  uint64_t bridges;          /* edges with bridge_out = 1                                          */
+  uint64_t components;       /* biconnected components (self-loops belong to none)                 */
+  uint64_t edges_inspected;  /* adjacency entries read, forest and low / high passes together      */
+  double run_ms;             /* CUDA-event time, first kernel .. last label written (no transfers) */
+  uint64_t kernel_launches;
+} mgb200_biconnectivity_stats;
+
+/* from / to: the host uint64 COO the graph was built from, in the same order (m must equal the graph's edge count).
+ * bridge_out: m uint8 values, bcc_out: m int64 values, both host memory; either may be NULL. */
+int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *from, const uint64_t *to,
+                              uint8_t *bridge_out, int64_t *bcc_out, mgb200_biconnectivity_stats *stats);
+
+/* One shot on device 0: host COO (uint64 endpoints < n) -> bridge_out[m] / bcc_out[m] in host memory. */
+int mgb200_bridges(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to, uint8_t *bridge_out);
+int mgb200_biconnected_components(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to, int64_t *bcc_out);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -42,6 +42,11 @@ class WccStats(ctypes.Structure):
                 ("run_ms", f64), ("kernel_launches", u64)]
 
 
+class BiconnectivityStats(ctypes.Structure):
+    _fields_ = [("trees", u64), ("forest_depth", u32), ("bridges", u64), ("components", u64), ("edges_inspected", u64),
+                ("run_ms", f64), ("kernel_launches", u64)]
+
+
 class KatzStats(ctypes.Structure):
     _fields_ = [("iterations", u64), ("max_out_degree", u64), ("gamma", f64), ("iterate_ms", f64),
                 ("kernel_launches", u64), ("tie_order_runs", u64)]
@@ -97,6 +102,9 @@ EXPORTS = {
     "mgb200_betweenness_centrality": (i32, [u64, u64, vp, vp, i32, i32, vp]),
     "mgb200_wcc_run": (i32, [vp, vp, ctypes.POINTER(WccStats)]),
     "mgb200_weakly_connected_components": (i32, [u64, u64, vp, vp, vp]),
+    "mgb200_biconnectivity_run": (i32, [vp, u64, vp, vp, vp, vp, ctypes.POINTER(BiconnectivityStats)]),
+    "mgb200_bridges": (i32, [u64, u64, vp, vp, vp]),
+    "mgb200_biconnected_components": (i32, [u64, u64, vp, vp, vp]),
     # include/mgb200_katz.h
     "mgb200_katz_run": (i32, [vp, f64, f64, u64, vp, ctypes.POINTER(KatzStats)]),
     "mgb200_katz_centrality": (i32, [u64, u64, vp, vp, f64, f64, u64, vp, ctypes.POINTER(u64)]),

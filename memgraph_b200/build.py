@@ -4,7 +4,8 @@
     memgraph_b200/_build/pagerank.so             drop-in Memgraph query module (mgp_init_module / mgp_shutdown_module)
     memgraph_b200/_build/libmgp_fake_host.so     fake mgp host used by the tests to load query modules without Memgraph
     memgraph_b200/_build/<module>.so             the other query modules (gpu_bfs, katz_centrality, betweenness_centrality,
-                                                 weakly_connected_components, cugraph.*), same linking as pagerank.so
+                                                 weakly_connected_components, bridges, biconnected_components,
+                                                 cugraph.*), same linking as pagerank.so
 
 Objects are rebuilt only when a source or header is newer.  `python -m memgraph_b200.build` builds everything.
 """
@@ -31,8 +32,9 @@ NVCC_FLAGS = [
     "-diag-suppress", "1444",  # cub::TransformInputIterator deprecation notice
 ]
 CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu",
-                "wcc.cu"]
+                "wcc.cu", "biconnectivity.cu"]
 HEADERS = [os.path.join(CSRC, "core.hpp"), os.path.join(CSRC, "bfs_graph.hpp"), os.path.join(CSRC, "rmat.hpp"), os.path.join(CSRC, "sell_stream.cuh"),
+           os.path.join(CSRC, "union_find.cuh"),
            os.path.join(INCLUDE, "mgb200_pagerank.h"), os.path.join(INCLUDE, "mgb200_bfs.h"),
            os.path.join(INCLUDE, "mgb200_katz.h"), os.path.join(INCLUDE, "mgb200_personalized.h"), os.path.join(CSRC, "katz_heap.hpp"),
            os.path.join(INCLUDE, "mgp_abi.h"), os.path.join(CSRC, "mgp_module_common.hpp")]
@@ -46,6 +48,7 @@ KATZ_MODULE_LIB = os.path.join(OUT, "katz_centrality.so")
 BC_MODULE_LIB = os.path.join(OUT, "betweenness_centrality.so")
 WCC_MODULE_LIB = os.path.join(OUT, "weakly_connected_components.so")
 WCC_HOST_LIB = os.path.join(OUT, "libmgp_wcc_host.so")
+EDGE_HOST_LIB = os.path.join(OUT, "libmgp_edge_host.so")
 
 
 def _newer(target, deps):
@@ -144,6 +147,25 @@ def build_wcc_module(objs, verbose=False):
         _run([NVCC, "-shared", "-cudart", "static", "-o", WCC_MODULE_LIB, obj] + objs)
 
 
+BICONNECTIVITY_MODULE_LIBS = {"bridges": os.path.join(OUT, "bridges.so"),
+                              "biconnected_components": os.path.join(OUT, "biconnected_components.so")}
+
+
+def build_biconnectivity_modules(objs, verbose=False):
+    """bridges.so / biconnected_components.so: bridges and biconnected components behind the reference modules' names
+    and signatures (one source, compiled twice; MGB200_BRIDGES selects the procedure)."""
+    src = os.path.join(CSRC, "biconnectivity_modules.cpp")
+    for name, lib in BICONNECTIVITY_MODULE_LIBS.items():
+        obj = os.path.join(OUT, f"{name}_module.o")
+        if _newer(obj, [src] + HEADERS):
+            if verbose:
+                print(f"g++ biconnectivity_modules.cpp ({name})", flush=True)
+            _run([CXX, "-std=c++20", "-O2", "-fPIC", "-fvisibility=hidden",
+                  f"-DMGB200_BRIDGES={1 if name == 'bridges' else 0}", "-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj])
+        if _newer(lib, objs + [obj]):
+            _run([NVCC, "-shared", "-cudart", "static", "-o", lib, obj] + objs)
+
+
 CUGRAPH_MODULE_LIBS = {0: os.path.join(OUT, "cugraph.pagerank.so"), 1: os.path.join(OUT, "cugraph.personalized_pagerank.so")}
 
 
@@ -194,6 +216,16 @@ def build_wcc_host(verbose=False):
         _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", WCC_HOST_LIB, WCC_HOST_SRC, "-ldl"])
 
 
+EDGE_HOST_SRC = os.path.join(REPO, "tests", "mgp_edge_host.cpp")  # the INTEGER host plus (node_from, node_to) rows
+
+
+def build_edge_host(verbose=False):
+    if _newer(EDGE_HOST_LIB, [EDGE_HOST_SRC, WCC_HOST_SRC, BC_HOST_SRC, FAKE_HOST_SRC] + HEADERS):
+        if verbose:
+            print("g++ mgp_edge_host.cpp", flush=True)
+        _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", EDGE_HOST_LIB, EDGE_HOST_SRC, "-ldl"])
+
+
 def build_all(verbose=False):
     objs = build_core(verbose)
     if os.path.exists(os.path.join(CSRC, "pagerank_module.cpp")):
@@ -216,6 +248,10 @@ def build_all(verbose=False):
     if os.path.exists(os.path.join(CSRC, "weakly_connected_components_module.cpp")):
         build_wcc_module(objs, verbose)
         out["weakly_connected_components_module"] = WCC_MODULE_LIB
+    if os.path.exists(os.path.join(CSRC, "biconnectivity_modules.cpp")):
+        build_biconnectivity_modules(objs, verbose)
+        for name, lib in BICONNECTIVITY_MODULE_LIBS.items():
+            out[name + "_module"] = lib
     if os.path.exists(os.path.join(CSRC, "gpu_bfs_module.cpp")):
         out["bfs_module"] = BFS_MODULE_LIB
     if os.path.exists(os.path.join(CSRC, "pagerank_module.cpp")):
@@ -228,6 +264,9 @@ def build_all(verbose=False):
     if os.path.exists(WCC_HOST_SRC):
         build_wcc_host(verbose)
         out["wcc_host"] = WCC_HOST_LIB
+    if os.path.exists(EDGE_HOST_SRC):
+        build_edge_host(verbose)
+        out["edge_host"] = EDGE_HOST_LIB
     return out
 
 

@@ -31,6 +31,7 @@
 #include "bfs_graph.hpp"
 #include "core.hpp"
 #include "mgb200_bfs.h"
+#include "union_find.cuh"
 
 namespace mgb200 {
 namespace {
@@ -56,23 +57,6 @@ struct Counters {
   unsigned int mid;    // vertices queued for a warp each (front of the work list)
   unsigned int heavy;  // vertices queued for a block each (back of the work list)
 };
-
-__device__ __forceinline__ uint32_t load(const uint32_t *parent, uint32_t i) {
-  return *(reinterpret_cast<const volatile uint32_t *>(parent) + i);  // other threads hook roots concurrently
-}
-
-// Union of the sets of u and v: the larger root is hooked under the smaller one.
-__device__ __forceinline__ void link(uint32_t u, uint32_t v, uint32_t *parent) {
-  uint32_t p1 = load(parent, u), p2 = load(parent, v);
-  while (p1 != p2) {
-    const uint32_t high = max(p1, p2), low = min(p1, p2);
-    const uint32_t p_high = load(parent, high);
-    if (p_high == low) break;  // already hooked there
-    if (p_high == high && atomicCAS(parent + high, high, low) == high) break;
-    p1 = load(parent, load(parent, high));
-    p2 = load(parent, low);
-  }
-}
 
 // Entry i of v's undirected list (i < out-degree + in-degree).
 __device__ __forceinline__ uint32_t entry(const Lists &g, uint64_t out_begin, uint64_t out_deg, uint64_t in_begin,
@@ -108,19 +92,6 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(uint64_t n, Lists g, u
     }
   }
   add_warp_sum(inspected, &counters->inspected);
-}
-
-// Every vertex points at its root afterwards.  Run only while no link is in flight.
-__global__ void __launch_bounds__(kThreads) compress_kernel(uint64_t n, uint32_t *parent) {
-  for (uint64_t v = first_thread(); v < n; v += thread_count()) {
-    const uint32_t p0 = parent[v];
-    uint32_t p = p0, pp = load(parent, p);
-    while (p != pp) {
-      p = pp;
-      pp = load(parent, p);
-    }
-    if (p != p0) parent[v] = p;
-  }
 }
 
 __device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser
