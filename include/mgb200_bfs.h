@@ -142,6 +142,65 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
 int mgb200_bridges(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to, uint8_t *bridge_out);
 int mgb200_biconnected_components(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to, int64_t *bcc_out);
 
+/*
+ * Weighted shortest paths from one source on the same device graph: the totals of the reference's
+ * `MATCH (a)-[*WSHORTEST ..u (e, n | e.w) total_weight]->(b)` with an unbound target and one numeric edge property as
+ * the weight (ExpandWeightedShortestPathCursor, src/query/plan/operator.cpp:2917-3267).
+ *
+ * Weights are doubles w >= +0 (+inf allowed; -0.0 is stored as +0.0).  A negative or NaN weight is an INVALID entry:
+ * it is stored as the quiet NaN 0x7FF8000000000000 | e, where e is the entry's index in the COO given to
+ * mgb200_bfs_graph_set_weights (e < 2^51).  Totals are left folds of IEEE round-to-nearest additions; because
+ * fl(a + w) is monotone in a and never below a, every relaxation order reaches the same least fixed point, so dist is
+ * bit-exact.  upper_bound == INT64_MAX is unbounded (delta-stepping); otherwise at most upper_bound Jacobi Bellman-Ford
+ * rounds give the minimum over walks of at most upper_bound edges.
+ *
+ * Output per vertex v (host memory):
+ *   dist_out[v] = v's total_weight (may be +inf), NaN when v is not produced (unreached, or the source itself);
+ *   hops_out[v] = the fewest edges among the paths the reference can return for v, -1 when v is not produced:
+ *                 unbounded, the BFS depth of v over tight entries (d[v] == fl(d[u] + w)); bounded, the smallest k with
+ *                 d_k[v] == d_upper_bound[v].
+ * If an entry the reference would evaluate (an entry of the walked direction out of a vertex that gets expanded) is
+ * invalid, the call returns MGB200_ERR_INVALID_WEIGHT and stats->invalid_edge holds the smallest COO index among the
+ * evaluated invalid entries; dist_out / hops_out are then unspecified.  Without a device every call fails with
+ * MGB200_ERR_CUDA.
+ */
+#define MGB200_ERR_INVALID_WEIGHT 17 /* an evaluated edge weight is negative or not a number */
+#define MGB200_WSP_UNBOUNDED INT64_MAX
+#define MGB200_WSP_INVALID_TAG 0x7FF8000000000000ull /* invalid entry = this | COO index */
+
+typedef struct mgb200_wsp_stats {
+  uint64_t rounds;             /* relaxation passes: Bellman-Ford rounds, or near-pile passes of all buckets      */
+  uint64_t buckets;            /* distance buckets processed (unbounded), 0 when bounded                          */
+  uint32_t hop_levels;         /* deepest hops value of a produced vertex                                         */
+  double delta;                /* bucket width (unbounded), 0 when bounded                                        */
+  uint64_t reached;            /* vertices produced                                                               */
+  uint64_t relaxations;        /* (pass, vertex) pairs whose distance a pass lowered                              */
+  uint64_t entries_inspected;  /* adjacency entries read, distance passes and the tight-entry BFS together        */
+  uint64_t invalid_edge;       /* smallest COO index of an evaluated invalid entry, UINT64_MAX when there is none */
+  double run_ms;               /* CUDA-event time, distance init .. last output written (no transfers)            */
+  uint64_t kernel_launches;
+} mgb200_wsp_stats;
+
+/* Weights of the COO the graph was built from (from / to / weight host arrays of m entries, m equal to the graph's
+ * edge count, same pairs in any order).  Builds out_w / in_w aligned with the sorted out- and in-lists; calling it
+ * again replaces them.  Duplicates of one (u, v) pair may take each other's weights: no answer depends on that.
+ * A COO whose (from, to) pairs differ from the graph's is refused with MGB200_ERR_INVALID_ARGUMENT.  Any failure
+ * leaves the graph without weights (never with a mix of the old and the new ones).  Device staging: 24 B per edge
+ * plus the sort's temporary, on top of the 16 B per edge the two weight arrays keep. */
+int mgb200_bfs_graph_set_weights(mgb200_bfs_graph *g, uint64_t m, const uint64_t *from, const uint64_t *to,
+                                 const double *weight);
+
+/* should_abort (may be NULL) is polled between host round trips; non-zero -> MGB200_ERR_ABORTED.  stats may be NULL.
+ * upper_bound < 1 -> MGB200_ERR_INVALID_ARGUMENT.  Two runs give byte-identical outputs and stats (run_ms aside). */
+int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t upper_bound,
+                   int (*should_abort)(void *user), void *abort_user, double *dist_out, int32_t *hops_out,
+                   mgb200_wsp_stats *stats);
+
+/* One shot on device 0: host COO with weights -> dist_out[n] / hops_out[n] in host memory. */
+int mgb200_weighted_shortest_paths(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to,
+                                   const double *weight, uint64_t source, int direction, int64_t upper_bound,
+                                   double *dist_out, int32_t *hops_out);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -47,6 +47,12 @@ class BiconnectivityStats(ctypes.Structure):
                 ("run_ms", f64), ("kernel_launches", u64)]
 
 
+class WspStats(ctypes.Structure):
+    _fields_ = [("rounds", u64), ("buckets", u64), ("hop_levels", u32), ("delta", f64), ("reached", u64),
+                ("relaxations", u64), ("entries_inspected", u64), ("invalid_edge", u64), ("run_ms", f64),
+                ("kernel_launches", u64)]
+
+
 class KatzStats(ctypes.Structure):
     _fields_ = [("iterations", u64), ("max_out_degree", u64), ("gamma", f64), ("iterate_ms", f64),
                 ("kernel_launches", u64), ("tie_order_runs", u64)]
@@ -63,6 +69,7 @@ class CugraphStats(ctypes.Structure):
 
 
 KATZ_NOT_CONVERGED = 16
+ERR_INVALID_WEIGHT = 17
 ABORT_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp)
 
 
@@ -105,6 +112,9 @@ EXPORTS = {
     "mgb200_biconnectivity_run": (i32, [vp, u64, vp, vp, vp, vp, ctypes.POINTER(BiconnectivityStats)]),
     "mgb200_bridges": (i32, [u64, u64, vp, vp, vp]),
     "mgb200_biconnected_components": (i32, [u64, u64, vp, vp, vp]),
+    "mgb200_bfs_graph_set_weights": (i32, [vp, u64, vp, vp, vp]),
+    "mgb200_wsp_run": (i32, [vp, u64, i32, ctypes.c_int64, ABORT_FN, vp, vp, vp, ctypes.POINTER(WspStats)]),
+    "mgb200_weighted_shortest_paths": (i32, [u64, u64, vp, vp, vp, u64, i32, ctypes.c_int64, vp, vp]),
     # include/mgb200_katz.h
     "mgb200_katz_run": (i32, [vp, f64, f64, u64, vp, ctypes.POINTER(KatzStats)]),
     "mgb200_katz_centrality": (i32, [u64, u64, vp, vp, f64, f64, u64, vp, ctypes.POINTER(u64)]),

@@ -5,7 +5,7 @@
     memgraph_b200/_build/libmgp_fake_host.so     fake mgp host used by the tests to load query modules without Memgraph
     memgraph_b200/_build/<module>.so             the other query modules (gpu_bfs, katz_centrality, betweenness_centrality,
                                                  weakly_connected_components, bridges, biconnected_components,
-                                                 cugraph.*), same linking as pagerank.so
+                                                 gpu_wsp, cugraph.*), same linking as pagerank.so
 
 Objects are rebuilt only when a source or header is newer.  `python -m memgraph_b200.build` builds everything.
 """
@@ -32,7 +32,7 @@ NVCC_FLAGS = [
     "-diag-suppress", "1444",  # cub::TransformInputIterator deprecation notice
 ]
 CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu",
-                "wcc.cu", "biconnectivity.cu"]
+                "wcc.cu", "biconnectivity.cu", "wsp.cu"]
 HEADERS = [os.path.join(CSRC, "core.hpp"), os.path.join(CSRC, "bfs_graph.hpp"), os.path.join(CSRC, "rmat.hpp"), os.path.join(CSRC, "sell_stream.cuh"),
            os.path.join(CSRC, "union_find.cuh"),
            os.path.join(INCLUDE, "mgb200_pagerank.h"), os.path.join(INCLUDE, "mgb200_bfs.h"),
@@ -49,6 +49,8 @@ BC_MODULE_LIB = os.path.join(OUT, "betweenness_centrality.so")
 WCC_MODULE_LIB = os.path.join(OUT, "weakly_connected_components.so")
 WCC_HOST_LIB = os.path.join(OUT, "libmgp_wcc_host.so")
 EDGE_HOST_LIB = os.path.join(OUT, "libmgp_edge_host.so")
+WSP_MODULE_LIB = os.path.join(OUT, "gpu_wsp.so")
+WSP_HOST_LIB = os.path.join(OUT, "libmgp_wsp_host.so")
 
 
 def _newer(target, deps):
@@ -147,6 +149,18 @@ def build_wcc_module(objs, verbose=False):
         _run([NVCC, "-shared", "-cudart", "static", "-o", WCC_MODULE_LIB, obj] + objs)
 
 
+def build_wsp_module(objs, verbose=False):
+    """gpu_wsp.so: the weighted shortest path expansion as a read procedure (same linking rules as pagerank.so)."""
+    src = os.path.join(CSRC, "gpu_wsp_module.cpp")
+    obj = os.path.join(OUT, "gpu_wsp_module.o")
+    if _newer(obj, [src] + HEADERS):
+        if verbose:
+            print("g++ gpu_wsp_module.cpp", flush=True)
+        _run([CXX, "-std=c++20", "-O2", "-fPIC", "-fvisibility=hidden", "-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj])
+    if _newer(WSP_MODULE_LIB, objs + [obj]):
+        _run([NVCC, "-shared", "-cudart", "static", "-o", WSP_MODULE_LIB, obj] + objs)
+
+
 BICONNECTIVITY_MODULE_LIBS = {"bridges": os.path.join(OUT, "bridges.so"),
                               "biconnected_components": os.path.join(OUT, "biconnected_components.so")}
 
@@ -226,6 +240,16 @@ def build_edge_host(verbose=False):
         _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", EDGE_HOST_LIB, EDGE_HOST_SRC, "-ldl"])
 
 
+WSP_HOST_SRC = os.path.join(REPO, "tests", "mgp_wsp_host.cpp")  # the base host plus a node / FLOAT / INTEGER call
+
+
+def build_wsp_host(verbose=False):
+    if _newer(WSP_HOST_LIB, [WSP_HOST_SRC, FAKE_HOST_SRC] + HEADERS):
+        if verbose:
+            print("g++ mgp_wsp_host.cpp", flush=True)
+        _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", WSP_HOST_LIB, WSP_HOST_SRC, "-ldl"])
+
+
 def build_all(verbose=False):
     objs = build_core(verbose)
     if os.path.exists(os.path.join(CSRC, "pagerank_module.cpp")):
@@ -252,6 +276,9 @@ def build_all(verbose=False):
         build_biconnectivity_modules(objs, verbose)
         for name, lib in BICONNECTIVITY_MODULE_LIBS.items():
             out[name + "_module"] = lib
+    if os.path.exists(os.path.join(CSRC, "gpu_wsp_module.cpp")):
+        build_wsp_module(objs, verbose)
+        out["wsp_module"] = WSP_MODULE_LIB
     if os.path.exists(os.path.join(CSRC, "gpu_bfs_module.cpp")):
         out["bfs_module"] = BFS_MODULE_LIB
     if os.path.exists(os.path.join(CSRC, "pagerank_module.cpp")):
@@ -267,6 +294,9 @@ def build_all(verbose=False):
     if os.path.exists(EDGE_HOST_SRC):
         build_edge_host(verbose)
         out["edge_host"] = EDGE_HOST_LIB
+    if os.path.exists(WSP_HOST_SRC):
+        build_wsp_host(verbose)
+        out["wsp_host"] = WSP_HOST_LIB
     return out
 
 

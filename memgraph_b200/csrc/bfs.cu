@@ -263,8 +263,8 @@ extern "C" {
 void mgb200_bfs_graph_destroy(mgb200_bfs_graph *g) {
   if (!g) return;
   cudaSetDevice(g->device);
-  void *ptrs[] = {g->out_ptr, g->in_ptr, g->out_adj, g->in_adj, g->depth, g->queue[0], g->queue[1], g->bitmap[0],
-                  g->bitmap[1], g->seg_count, g->seg_scan, g->counters, g->cub_tmp};
+  void *ptrs[] = {g->out_ptr, g->in_ptr, g->out_adj, g->in_adj, g->out_w, g->in_w, g->depth, g->queue[0], g->queue[1],
+                  g->bitmap[0], g->bitmap[1], g->seg_count, g->seg_scan, g->counters, g->cub_tmp};
   for (void *p : ptrs)
     if (p) cudaFree(p);
   if (g->host_counters) cudaFreeHost(g->host_counters);

@@ -1,6 +1,6 @@
 // memgraph_b200/csrc/bfs_graph.hpp -- the device graph behind the opaque mgb200_bfs_graph handle (include/mgb200_bfs.h).
-// Shared by the breadth-first expansion (bfs.cu), which builds it, betweenness centrality (betweenness.cu) and weakly
-// connected components (wcc.cu), which walk the same CSR + CSC.
+// Shared by the breadth-first expansion (bfs.cu), which builds it, betweenness centrality (betweenness.cu), weakly
+// connected components (wcc.cu) and weighted shortest paths (wsp.cu), which walk the same CSR + CSC.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -17,6 +17,9 @@ struct mgb200_bfs_graph {
   uint64_t n = 0, m = 0;
   uint64_t *out_ptr = nullptr, *in_ptr = nullptr;   // [n + 1]
   uint32_t *out_adj = nullptr, *in_adj = nullptr;   // [m], sorted inside a row
+  double *out_w = nullptr, *in_w = nullptr;         // [m] weights aligned with out_adj / in_adj; null until
+                                                    // mgb200_bfs_graph_set_weights (wsp.cu)
+  double mean_weight = 0.0;                         // mean of the finite valid weights (wsp.cu's bucket width)
   int32_t *depth = nullptr;                         // [n]
   uint32_t *queue[2] = {nullptr, nullptr};          // [n] frontier vertex lists
   uint32_t *bitmap[2] = {nullptr, nullptr};         // [ceil(n/32)]

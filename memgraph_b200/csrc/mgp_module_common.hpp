@@ -1,4 +1,4 @@
-// memgraph_b200/csrc/mgp_module_common.hpp -- host-side pieces shared by the query modules (pagerank.so, gpu_bfs.so):
+// memgraph_b200/csrc/mgp_module_common.hpp -- host-side pieces shared by the query modules (pagerank.so, gpu_bfs.so, ...):
 // mgp_error -> exception with the reference's texts, owning iterator wrappers, and the one-pass graph pull through
 // the mgp_graph iterators (the reference's CreatePageRankGraph, mage/cpp/pagerank_module/pagerank_module.cpp:18-54).
 #pragma once
@@ -9,6 +9,7 @@
 #include <exception>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "mgp_abi.h"
@@ -196,7 +197,13 @@ enum class UnknownGid { kUnknownToZero, kUnknownDropped };
 
 // The reference's ingest (CreatePageRankGraph :18-54): one vertex iterator, one out-edge iterator per
 // vertex, dense id = visit index, destinations remapped afterwards.
-inline HostGraph PullGraph(mgp_graph *graph, mgp_memory *memory, UnknownGid policy = UnknownGid::kUnknownToZero) {
+// Optional per-edge read in the same pass: `read(edge)` is called on every out-edge and its result lands in
+// `*edge_values`, kept in step with hg.from / hg.to (dropped edges drop their value too).  Without it (the default)
+// nothing is read and the function is the plain pull.
+template <typename Value = int, typename Read = std::nullptr_t>
+inline HostGraph PullGraph(mgp_graph *graph, mgp_memory *memory, UnknownGid policy = UnknownGid::kUnknownToZero,
+                           Read read = nullptr, std::vector<Value> *edge_values = nullptr) {
+  constexpr bool kRead = !std::is_same_v<Read, std::nullptr_t>;
   HostGraph hg;
   std::size_t approx_vertices = 0, approx_edges = 0;
   Check(mgp_graph_approximate_vertex_count(graph, &approx_vertices));
@@ -223,6 +230,7 @@ inline HostGraph PullGraph(mgp_graph *graph, mgp_memory *memory, UnknownGid poli
         Check(mgp_vertex_get_id(destination, &destination_id));
         hg.from.push_back(static_cast<uint32_t>(source_dense));
         to_gid.push_back(destination_id.as_int);
+        if constexpr (kRead) edge_values->push_back(read(edge));
       }
     }
     dense_of_gid.Put(source_id.as_int, source_dense);
@@ -240,10 +248,12 @@ inline HostGraph PullGraph(mgp_graph *graph, mgp_memory *memory, UnknownGid poli
     if (!known && policy == UnknownGid::kUnknownDropped) continue;
     hg.from[kept] = static_cast<uint32_t>(dense_of_gid.GetOrZero(hg.gid_of_dense[hg.from[e]]));
     hg.to[kept] = static_cast<uint32_t>(known ? dst : 0);
+    if constexpr (kRead) (*edge_values)[kept] = (*edge_values)[e];
     ++kept;
   }
   hg.from.resize(kept);
   hg.to.resize(kept);
+  if constexpr (kRead) edge_values->resize(kept);
   return hg;
 }
 
