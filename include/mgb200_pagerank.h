@@ -70,6 +70,8 @@ typedef struct mgb200_graph_info {
   uint64_t block_edges;    /* in-edges from labels >= MGB200_BLOCK_FROM (block class) */
   uint64_t block_chunks;   /* their (row, label block) runs, <= MGB200_BLOCK_CHUNK    */
   uint64_t blocks;         /* label blocks with at least one chunk (one launch each)  */
+  uint64_t tile_slices;    /* SELL-32 slices of tile chunks, tile-major               */
+  uint64_t tile_runs;      /* contiguous slice runs the tile kernel's CTAs draw (MGB200_TILE_RUNS) */
 } mgb200_graph_info;
 
 typedef struct mgb200_run_stats {

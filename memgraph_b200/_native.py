@@ -19,7 +19,8 @@ class GraphInfo(ctypes.Structure):
                 ("heavy_segments", u64), ("sell_rows", u64), ("sell_slices", u64), ("sell_entries", u64),
                 ("zero_rows", u64), ("resident_bytes", u64), ("build_ms", f64), ("upload_ms", f64), ("build_peak_bytes", u64),
                 ("tiled_edges", u64), ("tile_chunks", u64),
-                ("block_edges", u64), ("block_chunks", u64), ("blocks", u64)]
+                ("block_edges", u64), ("block_chunks", u64), ("blocks", u64),
+                ("tile_slices", u64), ("tile_runs", u64)]
 
 
 class RunStatsC(ctypes.Structure):

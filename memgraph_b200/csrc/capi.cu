@@ -617,6 +617,8 @@ int mgb200_graph_get_info(const mgb200_graph *h, mgb200_graph_info *info) {
   info->block_edges = g.block_edges;
   info->block_chunks = g.block_chunks;
   info->blocks = g.block_slice_first.empty() ? 0 : g.block_slice_first.size() - 1;
+  info->tile_slices = g.tile_slices;
+  info->tile_runs = g.tile_work;
   return MGB200_OK;
 }
 

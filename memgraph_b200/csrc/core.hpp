@@ -195,8 +195,9 @@ struct Graph {
   uint64_t *tslice_colbase = nullptr;   // [tile_slices + 1] in units of 32-entry columns
   uint16_t *tile_idx = nullptr;         // [32 * columns] offset of the source inside its tile
   uint64_t *tile_slot = nullptr;        // [32 * tile_slices] partial written by each lane; ~0 = padding lane
-  uint32_t tile_work = 0;               // work items = CTAs of heavy_tiles_kernel: contiguous slice runs, ~equal cost
+  uint32_t tile_work = 0;               // runs of heavy_tiles_kernel: contiguous slice runs, ~equal cost, several per SM
   uint64_t *tile_work_begin = nullptr;  // [tile_work + 1]
+  WorkQueue *tile_queue = nullptr;      // ticket of the runs (zero between launches)
   int tile_attr_bytes = 0;              // dynamic shared memory already granted to heavy_tiles_kernel
   // block class (one partition, unweighted; graph_build.cu steps 6b and 9).  A heavy row's in-edges from labels >=
   // block_from are summed one label block of block_labels labels at a time, so the block's part of contrib stays in L2

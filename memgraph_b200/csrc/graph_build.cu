@@ -649,6 +649,7 @@ void free_graph(Graph &g) {
   if (g.sell_work_begin) cudaFree(g.sell_work_begin);
   if (g.sell_work_items) cudaFree(g.sell_work_items);
   if (g.queue) cudaFree(g.queue);
+  if (g.tile_queue) cudaFree(g.tile_queue);
   if (g.sell_sums) cudaFree(g.sell_sums);
   if (g.out_stage) cudaFree(g.out_stage);
   if (g.need_mask) cudaFree(g.need_mask);
@@ -761,6 +762,8 @@ int build_graph(Graph &g, EdgeSource &edges) {
   MGB_CUDA(keep_alloc(g, &g.sum_partials, kSumBlocks));
   MGB_CUDA(keep_alloc(g, &g.queue, 1));
   MGB_CUDA(cudaMemsetAsync(g.queue, 0, sizeof(WorkQueue), st));
+  MGB_CUDA(keep_alloc(g, &g.tile_queue, 1));
+  MGB_CUDA(cudaMemsetAsync(g.tile_queue, 0, sizeof(WorkQueue), st));
   g.contrib_stride = ((n + 1) * sizeof(double) + 255) / 256 * 256;
   g.window_bytes = kFlagPageBytes + 2 * g.contrib_stride;
   MGB_CUDA(cudaMalloc(&g.window, g.window_bytes));
@@ -1202,8 +1205,12 @@ int build_graph(Graph &g, EdgeSource &edges) {
       tile_fill_kernel<<<blocks_for(ns * 32, g.sm_count), kThreads, 0, st>>>(
           ns, g.tslice_tile, g.tile_slice_first, d_chunk_first, g.tile_base, g.tslice_colbase, sorted_id, cbegin, clen,
           cslot, ekey, static_cast<uint16_t>(T), g.tile_idx, g.tile_slot);
-      // one work item per CTA (one CTA per SM): contiguous slice runs of ~equal cost = columns + 8 per slice
-      g.tile_work = static_cast<uint32_t>(std::min<uint64_t>(ns, g.sm_count));
+      // runs of heavy_tiles_kernel: contiguous slice runs of ~equal cost = columns + 8 per slice, drawn in tile order by
+      // one persistent CTA per SM.  8 runs per SM (MGB200_TILE_RUNS sets the total): scale-26 on one H100, one
+      // bench.py --quick run each, 4 per SM is slower (8.46 against 8.32 ms per iteration) and 16 is not faster (8.34);
+      // a slice cost of 2 is slower (8.41), 24 no faster (8.31), so the SELL items' 8 stays.
+      g.tile_work = static_cast<uint32_t>(
+          std::min<uint64_t>(ns, env_u32("MGB200_TILE_RUNS", static_cast<uint32_t>(g.sm_count) * 8u)));
       MGB_CUDA(keep_alloc(g, &g.tile_work_begin, static_cast<uint64_t>(g.tile_work) + 1));
       sell_items_kernel<<<(g.tile_work + 1 + kThreads - 1) / kThreads, kThreads, 0, st>>>(
           g.tile_work, ns, g.tslice_colbase, total_cols, 8, g.tile_work_begin);

@@ -573,9 +573,10 @@ __global__ void __launch_bounds__(kTableThreads, 1) sell_rows_table_kernel(const
 
 // Tile chunks (graph_build.cu 7c): a CTA copies one tile of contrib into shared memory with TMA bulk copies and serves
 // every chunk of that tile from it -- per edge a 2-byte offset and a shared-memory read instead of a 4-byte index and
-// an L2 request.  Slices are tile-major, and each CTA walks ONE contiguous run of them (its work item), so it refills
-// only where its run crosses into the next tile: about (tiles + CTAs) fills per launch.  Inside a tile, the CTA's warps
-// draw slices from a shared counter; a lane adds its chunk in ascending source order and writes the chunk's partial.
+// an L2 request.  Slices are tile-major and cut into RUNS of about equal cost, several per SM; one persistent CTA per SM
+// draws runs from a ticket in tile order, so a CTA that drew cheap runs simply takes more, and its next run lies in the
+// tile it holds or in a later one (it refills only when the tile changes).  Inside a run the CTA's warps draw GROUPS of
+// consecutive slices from a shared counter and walk each group as one stream of columns (tile_walk).
 struct TileArgs {
   const uint16_t *idx;          // [32 * columns] tile offsets, column-major per slice
   const uint64_t *colbase;      // [slices + 1]
@@ -583,25 +584,114 @@ struct TileArgs {
   const uint64_t *slot;         // [32 * slices] partial of each lane's chunk, ~0 = padding lane
   const uint64_t *tile_slice_first;  // [tiles + 1]
   const uint32_t *tile_base, *tile_load;  // [tiles] first label (even) and labels copied (even)
-  const uint64_t *work_begin;   // [n_work + 1]
+  const uint64_t *work_begin;   // [n_work + 1] first slice of every run
   uint32_t n_work;
+  WorkQueue *queue;             // ticket of the runs (rewound by the last CTA to leave)
   uint32_t tile_labels;         // T: shared slot T holds the 0.0 every padding offset reads
   const double *contrib_in;
   double *seg_partial;
   IterState *state;
 };
 constexpr int kTileThreads = 512;
+constexpr int kTileWarps = kTileThreads / 32;
 constexpr int kTileUnroll = 16;
+constexpr int kTileGroupMax = 31;     // slices per group: its column bases, both ends included, fill one warp-wide load
+constexpr int kTileGroupsPerWarp = 4; // groups a warp draws from a run's part of one tile, on average
 constexpr int kTileEpiCtas = 2;  // CTAs per SM of the side-stream SELL epilogue next to heavy_tiles_kernel
 __device__ __forceinline__ uint16_t ld_index16(const uint16_t *p, uint64_t pol) {
   uint16_t v;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u16 %0, [%1], %2;" : "=h"(v) : "l"(p), "l"(pol));
   return v;
 }
+__device__ __forceinline__ uint64_t ld_slot(const uint64_t *p, uint64_t pol) {
+  uint64_t v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol));
+  return v;
+}
+
+// One warp's share of slices [.., run_end) of the loaded tile.  A ticket on `next_slice` hands out a group of `group`
+// consecutive slices, which is one contiguous span of tile_idx because colbase is monotone; the warp walks the span as
+// ONE stream of columns (offset batch k+1 travels while batch k is summed), and a slice boundary only decides where the
+// lane's sum is stored -- narrow slices cost columns, not round trips.  The next group's ticket and column bases travel
+// while the current group is summed, and a slice's partial slots are requested two slices ahead.  A lane still adds its
+// chunk alone, from 0.0, in ascending source order: the partials are the bits a slice-by-slice walk gives.
+__device__ __forceinline__ void tile_walk(const TileArgs &a, const double *tile, unsigned long long *next_slice,
+                                          uint64_t run_end, uint32_t group, int lane, uint64_t pol) {
+  auto draw = [&]() -> uint64_t {
+    unsigned long long t = 0;
+    if (lane == 0) t = atomicAdd(next_slice, static_cast<unsigned long long>(group));
+    return __shfl_sync(kFull, t, 0);
+  };
+  // lane l: colbase[first + l], up to the end of the group's last slice
+  auto bases = [&](uint64_t first) -> uint64_t {
+    return (first < run_end && first + lane <= min(first + group, run_end)) ? a.colbase[first + lane] : 0ull;
+  };
+  auto slot_of = [&](uint64_t s, uint64_t end) -> uint64_t {
+    return s < end ? ld_slot(a.slot + s * kSliceRows + lane, pol) : ~0ull;
+  };
+  uint64_t my = draw();
+  uint64_t base = bases(my);
+  while (my < run_end) {
+    const uint64_t my_next = draw();
+    const uint64_t base_next = bases(my_next);
+    const uint64_t my_end = min(my + group, run_end);
+    const uint64_t c0 = __shfl_sync(kFull, base, 0);
+    const uint32_t ncols = static_cast<uint32_t>(__shfl_sync(kFull, base, static_cast<int>(my_end - my)) - c0);
+    const uint32_t rel = static_cast<uint32_t>(base - c0);  // lane l: first column of slice my + l, from the group's start
+    const uint16_t *p = a.idx + c0 * kSliceRows + lane;
+    uint16_t nxt[kTileUnroll];
+#pragma unroll
+    for (int j = 0; j < kTileUnroll; ++j)
+      if (static_cast<uint32_t>(j) < ncols) nxt[j] = ld_index16(p + static_cast<size_t>(j) * kSliceRows, pol);
+    uint64_t s = my;
+    uint64_t slot = slot_of(s, my_end), slot_ahead = slot_of(s + 1, my_end);
+    uint32_t slice_end = __shfl_sync(kFull, rel, 1);
+    double acc = 0.0;
+    // column `col` (group-relative, one past the column just added) closes every slice that ends there
+    auto close_slices = [&](uint32_t col) {
+      while (col == slice_end) {  // every slice is >= 1 column wide (its longest chunk has an edge), so col >= 1 suffices
+        if (slot != ~0ull) a.seg_partial[slot] = acc;
+        acc = 0.0;
+        ++s;
+        slot = slot_ahead;
+        slot_ahead = slot_of(s + 1, my_end);
+        slice_end = s < my_end ? __shfl_sync(kFull, rel, static_cast<int>(s - my) + 1) : 0xFFFFFFFFu;
+      }
+    };
+    for (uint32_t k = 0; k < ncols; k += kTileUnroll) {
+      uint16_t off[kTileUnroll];
+#pragma unroll
+      for (int j = 0; j < kTileUnroll; ++j) off[j] = nxt[j];
+#pragma unroll
+      for (int j = 0; j < kTileUnroll; ++j)  // the next batch of offsets travels while this batch is summed
+        if (k + kTileUnroll + j < ncols) nxt[j] = ld_index16(p + static_cast<size_t>(k + kTileUnroll + j) * kSliceRows, pol);
+      if (k + kTileUnroll <= slice_end) {  // the whole batch lies inside the current slice
+#pragma unroll
+        for (int j = 0; j < kTileUnroll; ++j) acc += tile[off[j]];  // ascending source order inside the chunk
+        close_slices(k + kTileUnroll);
+      } else {
+#pragma unroll
+        for (int j = 0; j < kTileUnroll; ++j) {
+          if (k + j < ncols) {
+            acc += tile[off[j]];
+            close_slices(k + j + 1);
+          }
+        }
+      }
+    }
+    my = my_next;
+    base = base_next;
+  }
+}
+
 __global__ void __launch_bounds__(kTileThreads, 2) heavy_tiles_kernel(const TileArgs a) {  // <= 64 registers
   extern __shared__ __align__(128) unsigned char tile_smem[];
   __shared__ __align__(8) unsigned long long fill_bar;
   __shared__ unsigned long long next_slice;
+  __shared__ uint32_t cta_run;
+  // `done` is written by iter_end_kernel and, when a peer barrier times out, by barrier_kernel; both run on this
+  // launch's stream, so every CTA of a launch reads the same value: either all of them draw tickets and count
+  // themselves out below, or none touches the queue
   if (ld_volatile_int(&a.state->done)) return;
   const double *tile = reinterpret_cast<const double *>(tile_smem);
   const int lane = threadIdx.x & 31;
@@ -611,10 +701,14 @@ __global__ void __launch_bounds__(kTileThreads, 2) heavy_tiles_kernel(const Tile
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     reinterpret_cast<double *>(tile_smem)[a.tile_labels] = 0.0;  // never overwritten: a fill copies <= T labels
   }
-  __syncthreads();
   const uint64_t pol = make_evict_first_policy();
   uint32_t phase = 0, cur_tile = 0xFFFFFFFFu;
-  for (uint32_t w = blockIdx.x; w < a.n_work; w += gridDim.x) {
+  while (true) {
+    if (threadIdx.x == 0)
+      cta_run = static_cast<uint32_t>(min(atomicAdd(&a.queue->ticket, 1ull), static_cast<unsigned long long>(a.n_work)));
+    __syncthreads();  // (first trip: the barrier is initialised before anyone waits on it)
+    const uint32_t w = cta_run;
+    if (w >= a.n_work) break;
     uint64_t s = a.work_begin[w];
     const uint64_t s_end = a.work_begin[w + 1];
     while (s < s_end) {
@@ -640,34 +734,22 @@ __global__ void __launch_bounds__(kTileThreads, 2) heavy_tiles_kernel(const Tile
         phase ^= 1u;
         cur_tile = t;
       }
-      while (true) {
-        unsigned long long my = 0;
-        if (lane == 0) my = atomicAdd(&next_slice, 1ull);
-        my = __shfl_sync(kFull, my, 0);
-        if (my >= run_end) break;
-        const uint64_t c0 = a.colbase[my], ncols = a.colbase[my + 1] - c0;
-        const uint64_t slot = a.slot[my * kSliceRows + lane];
-        const uint16_t *p = a.idx + c0 * kSliceRows + lane;
-        double acc = 0.0;
-        uint16_t nxt[kTileUnroll];
-#pragma unroll
-        for (int j = 0; j < kTileUnroll; ++j)
-          if (static_cast<uint64_t>(j) < ncols) nxt[j] = ld_index16(p + static_cast<size_t>(j) * kSliceRows, pol);
-        for (uint64_t k = 0; k < ncols; k += kTileUnroll) {
-          uint16_t off[kTileUnroll];
-#pragma unroll
-          for (int j = 0; j < kTileUnroll; ++j) off[j] = nxt[j];
-#pragma unroll
-          for (int j = 0; j < kTileUnroll; ++j)  // the next batch of offsets travels while this batch is summed
-            if (k + kTileUnroll + j < ncols) nxt[j] = ld_index16(p + static_cast<size_t>(k + kTileUnroll + j) * kSliceRows, pol);
-#pragma unroll
-          for (int j = 0; j < kTileUnroll; ++j)
-            if (k + j < ncols) acc += tile[off[j]];  // ascending source order inside the chunk
-        }
-        if (slot != ~0ull) a.seg_partial[slot] = acc;
-      }
-      __syncthreads();  // every warp is done with this run (and with next_slice) before the next fill
+      // enough groups that the warps finish this part of the run together, few enough that a group is a long stream
+      const uint32_t group = static_cast<uint32_t>(
+          min(static_cast<uint64_t>(kTileGroupMax), max(uint64_t{1}, (run_end - s) / (kTileWarps * kTileGroupsPerWarp))));
+      tile_walk(a, tile, &next_slice, run_end, group, lane, pol);
+      __syncthreads();  // every warp is done with this part (and with next_slice) before the next fill
       s = run_end;
+    }
+    __syncthreads();  // every thread has read cta_run before the next ticket overwrites it (an empty run has no part)
+  }
+  // the last CTA to leave rewinds the ticket for the next launch (every run of this launch has been drawn by then)
+  if (threadIdx.x == 0) {
+    const unsigned int left = atomicAdd(&a.queue->ctas_done, 1u);
+    if (left == gridDim.x - 1) {
+      a.queue->ticket = 0ull;
+      a.queue->ctas_done = 0u;
+      __threadfence();
     }
   }
 }
@@ -1228,15 +1310,16 @@ int launch_heavy_partials(Graph &g, const HeavyArgs &h, uint64_t reserve_ctas, u
     MGB_CUDA(cudaStreamWaitEvent(g.cold_stream, g.cold_fork_ev, 0));
   }
   if (g.tile_slices > 0) {
-    const TileArgs t{g.tile_idx,   g.tslice_colbase, g.tslice_tile,     g.tile_slot, g.tile_slice_first,
-                     g.tile_base,  g.tile_load,      g.tile_work_begin, g.tile_work, g.tun.tile_labels,
-                     h.contrib_in, g.seg_partial,    g.state};
+    const TileArgs t{g.tile_idx,   g.tslice_colbase, g.tslice_tile,     g.tile_slot,  g.tile_slice_first,
+                     g.tile_base,  g.tile_load,      g.tile_work_begin, g.tile_work,  g.tile_queue,
+                     g.tun.tile_labels, h.contrib_in, g.seg_partial,    g.state};
     const int bytes = static_cast<int>((g.tun.tile_labels + 1) * sizeof(double));
     if (g.tile_attr_bytes < bytes) {
       MGB_CUDA(cudaFuncSetAttribute(heavy_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
       g.tile_attr_bytes = bytes;
     }
-    heavy_tiles_kernel<<<g.tile_work, kTileThreads, bytes, g.stream>>>(t);
+    const uint32_t grid = std::min<uint32_t>(g.tile_work, static_cast<uint32_t>(g.sm_count));
+    heavy_tiles_kernel<<<grid, kTileThreads, bytes, g.stream>>>(t);
     MGB_CUDA(cudaGetLastError());
     ++*launches;
   }
