@@ -152,7 +152,8 @@ int mgb200_biconnected_components(uint64_t n, uint64_t m, const uint64_t *from, 
  * mgb200_bfs_graph_set_weights (e < 2^51).  Totals are left folds of IEEE round-to-nearest additions; because
  * fl(a + w) is monotone in a and never below a, every relaxation order reaches the same least fixed point, so dist is
  * bit-exact.  upper_bound == INT64_MAX is unbounded (delta-stepping); otherwise at most upper_bound Jacobi Bellman-Ford
- * rounds give the minimum over walks of at most upper_bound edges.
+ * rounds give the minimum over walks of at most upper_bound edges.  The environment variable MGB200_WSP_DELTA, read at
+ * every unbounded call, sets the bucket width when it is a finite number > 0; the width changes the work, not dist.
  *
  * Output per vertex v (host memory):
  *   dist_out[v] = v's total_weight (may be +inf), NaN when v is not produced (unreached, or the source itself);

@@ -34,6 +34,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdint>
+#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -454,6 +455,13 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
                              static_cast<double>(std::max<uint64_t>(n, 1));
   double delta = 32.0 * g->mean_weight / std::max(1.0, mean_degree);
   if (!(delta > 0.0) || !std::isfinite(delta)) delta = 1.0;
+  // MGB200_WSP_DELTA: a finite width > 0 replaces the heuristic (anything else is ignored).  The width changes the
+  // work only, never a result, so tests use it to put distances on bucket ends and to force many or one bucket.
+  if (const char *s = std::getenv("MGB200_WSP_DELTA")) {
+    char *end = nullptr;
+    const double v = std::strtod(s, &end);
+    if (end != s && *end == '\0' && v > 0.0 && std::isfinite(v)) delta = v;
+  }
 
   Buffers buf;
   uint64_t *dist = nullptr, *near_d[2] = {nullptr, nullptr};
