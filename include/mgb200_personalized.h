@@ -64,6 +64,61 @@ int mgb200_graph_create_host_weighted_u32(int device, uint64_t n, uint64_t m, co
 int mgb200_cugraph_pagerank_run(mgb200_graph *g, const mgb200_cugraph_params *params, double *rank_out,
                                 mgb200_cugraph_stats *stats);
 
+/* ---- HITS hubs and authorities (what the reference's cugraph.hits.get computes) ----------------------------------
+ *
+ *   reference call site                                                        replaced by
+ *   -------------------------------------------------------------------------  --------------------------------
+ *   cugraph::hits(handle, view, hubs, authorities, tolerance, max_iterations,    mgb200_hits_run()
+ *     false, normalize, false)   mage/cpp/cugraph_module/algorithms/hits.cu
+ *
+ * The arithmetic is rapidsai/cugraph's (third party, absent from the reference checkout; restated in
+ * oracle/cugraph_hits_oracle.c and pinned on the reference's e2e fixtures mage/tests/e2e/hits_test/test_cugraph_*):
+ *   prev = 1/N everywhere
+ *   repeat: auth[v] = sum_{u->v} prev[u];  auth /= max(auth)
+ *           hubs[u] = sum_{u->v} auth[v];  hubs /= max(hubs)
+ *           diff = sum_v |hubs[v] - prev[v]|;  ++iterations
+ *           stop when diff < N * tolerance (converged) or iterations >= max_iterations (not converged);  prev = hubs
+ *   normalized: hubs /= sum(hubs), auth /= sum(auth)
+ * Multi-edges count with multiplicity, self-loops count, edge weights play no part.  N is node_count: a vertex without
+ * edges ends with 0 in both vectors but counts in N (the query module passes only the vertices that occur in an edge,
+ * as cuGraph's renumbering does).  Two choices the fixtures do not decide:
+ *   - after max_iterations without convergence the last iterate is returned with stats.converged = 0 (no error);
+ *   - max_iterations = 0 runs one iteration; the module's negative INTEGER wraps through size_t and runs to convergence.
+ * A graph with n > 0 and no edges returns all zeros, converged = 1 and 0 iterations.
+ * Device side (hits.cu): the graph is built twice from one COO -- the forward handle gathers auth = A^T hubs, the
+ * reverse handle (the same COO with the endpoints swapped) gathers hubs = A auth -- with PageRank's layout and gather
+ * kernels on each.  Every reduction is two-stage with a fixed tree: results are bit-reproducible run to run and under
+ * every gather variant.  Single partition only.  No CPU fallback. */
+
+typedef struct mgb200_hits_graph mgb200_hits_graph; /* forward + reverse handles of one COO, one device */
+
+typedef struct mgb200_hits_params {
+  uint64_t max_iterations; /* module default 100 */
+  double tolerance;        /* module default 1e-5; the stop test is diff < node_count * tolerance */
+  int normalized;          /* module default true: both vectors scaled to sum 1 */
+} mgb200_hits_params;
+
+typedef struct mgb200_hits_stats {
+  uint64_t iterations;
+  int converged;            /* 0: max_iterations ended the loop */
+  double last_diff_sum;     /* L1 distance of the last two hub iterates (both max-scaled) */
+  double iterate_ms;        /* CUDA-event time of the loop and the output writes */
+  uint64_t kernel_launches;
+} mgb200_hits_stats;
+
+/* One COO (dense 32-bit ids < n, host memory), both directions built on `device`. */
+int mgb200_hits_graph_create_host_u32(int device, uint64_t n, uint64_t m, const uint32_t *from, const uint32_t *to,
+                                      mgb200_hits_graph **out);
+/* Layout of the forward handle (rows = in-edges: authorities) and of the reverse one (rows = out-edges: hubs). */
+int mgb200_hits_graph_get_info(const mgb200_hits_graph *g, mgb200_graph_info *forward, mgb200_graph_info *reverse);
+void mgb200_hits_graph_destroy(mgb200_hits_graph *g);
+/* hubs_out / authorities_out: node_count doubles each, HOST memory, original vertex-id order. */
+int mgb200_hits_run(mgb200_hits_graph *g, const mgb200_hits_params *params, double *hubs_out, double *authorities_out,
+                    mgb200_hits_stats *stats);
+/* Create + run + destroy on device MGB200_DEVICE (default 0). */
+int mgb200_hits(uint64_t n, uint64_t m, const uint32_t *from, const uint32_t *to, const mgb200_hits_params *params,
+                double *hubs_out, double *authorities_out, mgb200_hits_stats *stats);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -69,6 +69,15 @@ class CugraphStats(ctypes.Structure):
                 ("kernel_launches", u64)]
 
 
+class HitsParams(ctypes.Structure):
+    _fields_ = [("max_iterations", u64), ("tolerance", f64), ("normalized", i32)]
+
+
+class HitsStats(ctypes.Structure):
+    _fields_ = [("iterations", u64), ("converged", i32), ("last_diff_sum", f64), ("iterate_ms", f64),
+                ("kernel_launches", u64)]
+
+
 KATZ_NOT_CONVERGED = 16
 ERR_INVALID_WEIGHT = 17
 ABORT_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp)
@@ -123,6 +132,11 @@ EXPORTS = {
     # include/mgb200_personalized.h
     "mgb200_graph_create_host_weighted_u32": (i32, [i32, u64, u64, vp, vp, vp, ctypes.POINTER(vp)]),
     "mgb200_cugraph_pagerank_run": (i32, [vp, ctypes.POINTER(CugraphParams), vp, ctypes.POINTER(CugraphStats)]),
+    "mgb200_hits_graph_create_host_u32": (i32, [i32, u64, u64, vp, vp, ctypes.POINTER(vp)]),
+    "mgb200_hits_graph_get_info": (i32, [vp, ctypes.POINTER(GraphInfo), ctypes.POINTER(GraphInfo)]),
+    "mgb200_hits_graph_destroy": (None, [vp]),
+    "mgb200_hits_run": (i32, [vp, ctypes.POINTER(HitsParams), vp, vp, ctypes.POINTER(HitsStats)]),
+    "mgb200_hits": (i32, [u64, u64, vp, vp, ctypes.POINTER(HitsParams), vp, vp, ctypes.POINTER(HitsStats)]),
     "mgb200_graph_create_rmat": (i32, [i32, u32, u64, u64, f64, f64, f64, u32, u32, ctypes.POINTER(vp)]),
     "mgb200_rmat_generate_device": (i32, [i32, u32, u64, u64, u64, f64, f64, f64, vp, vp]),
     "mgb200_rmat_generate_host": (i32, [u32, u64, u64, u64, f64, f64, f64, vp, vp]),

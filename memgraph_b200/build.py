@@ -5,7 +5,8 @@
     memgraph_b200/_build/libmgp_fake_host.so     fake mgp host used by the tests to load query modules without Memgraph
     memgraph_b200/_build/<module>.so             the other query modules (gpu_bfs, katz_centrality, betweenness_centrality,
                                                  weakly_connected_components, bridges, biconnected_components,
-                                                 gpu_wsp, cugraph.*), same linking as pagerank.so
+                                                 gpu_wsp, cugraph.* including cugraph.hits), same linking
+                                                 as pagerank.so
 
 Objects are rebuilt only when a source or header is newer.  `python -m memgraph_b200.build` builds everything.
 """
@@ -32,7 +33,7 @@ NVCC_FLAGS = [
     "-diag-suppress", "1444",  # cub::TransformInputIterator deprecation notice
 ]
 CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu",
-                "wcc.cu", "biconnectivity.cu", "wsp.cu"]
+                "wcc.cu", "biconnectivity.cu", "wsp.cu", "hits.cu"]
 HEADERS = [os.path.join(CSRC, "core.hpp"), os.path.join(CSRC, "bfs_graph.hpp"), os.path.join(CSRC, "rmat.hpp"), os.path.join(CSRC, "sell_stream.cuh"),
            os.path.join(CSRC, "union_find.cuh"),
            os.path.join(INCLUDE, "mgb200_pagerank.h"), os.path.join(INCLUDE, "mgb200_bfs.h"),
@@ -181,19 +182,23 @@ def build_biconnectivity_modules(objs, verbose=False):
 
 
 CUGRAPH_MODULE_LIBS = {0: os.path.join(OUT, "cugraph.pagerank.so"), 1: os.path.join(OUT, "cugraph.personalized_pagerank.so")}
+CUGRAPH_HITS_MODULE_LIB = os.path.join(OUT, "cugraph.hits.so")
 
 
 def build_cugraph_modules(objs, verbose=False):
-    """cugraph.pagerank.so / cugraph.personalized_pagerank.so: stand-ins for the reference's cuGraph PageRank modules
-    (one source, compiled twice; module name = file stem, so the procedures are cugraph.pagerank.get and
-    cugraph.personalized_pagerank.get)."""
+    """cugraph.pagerank.so / cugraph.personalized_pagerank.so / cugraph.hits.so: stand-ins for the reference's cuGraph
+    PageRank and HITS modules (one source, compiled three times; module name = file stem, so the procedures are
+    cugraph.pagerank.get, cugraph.personalized_pagerank.get and cugraph.hits.get)."""
     src = os.path.join(CSRC, "cugraph_modules.cpp")
-    for personalized, lib in CUGRAPH_MODULE_LIBS.items():
-        obj = os.path.join(OUT, f"cugraph_module_{personalized}.o")
+    variants = [(f"cugraph_module_{p}.o", f"-DMGB200_CUGRAPH_PERSONALIZED={p}", lib, f"personalized={p}")
+                for p, lib in CUGRAPH_MODULE_LIBS.items()]
+    variants.append(("cugraph_module_hits.o", "-DMGB200_CUGRAPH_HITS=1", CUGRAPH_HITS_MODULE_LIB, "hits"))
+    for obj_name, define, lib, label in variants:
+        obj = os.path.join(OUT, obj_name)
         if _newer(obj, [src] + HEADERS):
             if verbose:
-                print(f"g++ cugraph_modules.cpp (personalized={personalized})", flush=True)
-            _run([CXX, "-std=c++20", "-O2", "-fPIC", "-fvisibility=hidden", f"-DMGB200_CUGRAPH_PERSONALIZED={personalized}",
+                print(f"g++ cugraph_modules.cpp ({label})", flush=True)
+            _run([CXX, "-std=c++20", "-O2", "-fPIC", "-fvisibility=hidden", define,
                   "-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj])
         if _newer(lib, objs + [obj]):
             _run([NVCC, "-shared", "-cudart", "static", "-o", lib, obj] + objs)
@@ -241,6 +246,8 @@ def build_edge_host(verbose=False):
 
 
 WSP_HOST_SRC = os.path.join(REPO, "tests", "mgp_wsp_host.cpp")  # the base host plus a node / FLOAT / INTEGER call
+HITS_HOST_SRC = os.path.join(REPO, "tests", "mgp_hits_host.cpp")  # the BOOLEAN host plus a call with named FLOAT columns
+HITS_HOST_LIB = os.path.join(OUT, "libmgp_hits_host.so")
 
 
 def build_wsp_host(verbose=False):
@@ -248,6 +255,13 @@ def build_wsp_host(verbose=False):
         if verbose:
             print("g++ mgp_wsp_host.cpp", flush=True)
         _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", WSP_HOST_LIB, WSP_HOST_SRC, "-ldl"])
+
+
+def build_hits_host(verbose=False):
+    if _newer(HITS_HOST_LIB, [HITS_HOST_SRC, BC_HOST_SRC, FAKE_HOST_SRC] + HEADERS):
+        if verbose:
+            print("g++ mgp_hits_host.cpp", flush=True)
+        _run([CXX, "-std=c++20", "-O2", "-fPIC", "-shared", "-I", INCLUDE, "-o", HITS_HOST_LIB, HITS_HOST_SRC, "-ldl"])
 
 
 def build_all(verbose=False):
@@ -263,6 +277,7 @@ def build_all(verbose=False):
         build_cugraph_modules(objs, verbose)
         out["cugraph_pagerank_module"] = CUGRAPH_MODULE_LIBS[0]
         out["cugraph_personalized_pagerank_module"] = CUGRAPH_MODULE_LIBS[1]
+        out["cugraph_hits_module"] = CUGRAPH_HITS_MODULE_LIB
     if os.path.exists(os.path.join(CSRC, "katz_centrality_module.cpp")):
         build_katz_module(objs, verbose)
         out["katz_module"] = KATZ_MODULE_LIB
@@ -297,6 +312,9 @@ def build_all(verbose=False):
     if os.path.exists(WSP_HOST_SRC):
         build_wsp_host(verbose)
         out["wsp_host"] = WSP_HOST_LIB
+    if os.path.exists(HITS_HOST_SRC):
+        build_hits_host(verbose)
+        out["hits_host"] = HITS_HOST_LIB
     return out
 
 

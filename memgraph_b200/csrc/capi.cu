@@ -251,7 +251,22 @@ int iterate(Graph &g, const mgb200_run_params &p, mgb200_run_stats &stats) {
 namespace mgb200 {
 int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double *d_out_original_order,
                              mgb200_cugraph_stats *stats);
+// hits.cu
+int hits_permutations(Graph &f, Graph &t, uint32_t *t_of_f, uint32_t *f_of_t);
+uint64_t hits_scratch_doubles(uint64_t n);
+int hits_iterate(Graph &f, Graph &t, const uint32_t *t_of_f, const uint32_t *f_of_t, const mgb200_hits_params &prm,
+                 double *scratch, cudaEvent_t f_done, cudaEvent_t t_done, double *d_hubs, double *d_auth,
+                 mgb200_hits_stats *stats);
 }
+
+// Both directions of one COO: fwd gathers along in-edges (authorities), rev along out-edges (hubs).
+struct mgb200_hits_graph {
+  mgb200::Graph fwd, rev;
+  uint32_t *t_of_f = nullptr, *f_of_t = nullptr;  // [n] each: label of a vertex in the other handle
+  double *scratch = nullptr;                       // hits_scratch_doubles(n)
+  double *out_stage = nullptr;                     // [2n] hubs, authorities in original order
+  cudaEvent_t f_done = nullptr, t_done = nullptr;  // orders the two handles' streams inside an iteration
+};
 
 using namespace mgb200;
 
@@ -592,9 +607,10 @@ void mgb200_graph_destroy(mgb200_graph *g) {
   delete g;
 }
 
-int mgb200_graph_get_info(const mgb200_graph *h, mgb200_graph_info *info) {
-  if (!h || !info) return MGB200_ERR_INVALID_ARGUMENT;
-  const Graph &g = h->g;
+}  // extern "C"
+
+namespace {
+void fill_info(const Graph &g, mgb200_graph_info *info) {
   info->node_count = g.n;
   info->edge_count = g.m;
   info->part_rank = g.part_rank;
@@ -619,6 +635,14 @@ int mgb200_graph_get_info(const mgb200_graph *h, mgb200_graph_info *info) {
   info->blocks = g.block_slice_first.empty() ? 0 : g.block_slice_first.size() - 1;
   info->tile_slices = g.tile_slices;
   info->tile_runs = g.tile_work;
+}
+}  // namespace
+
+extern "C" {
+
+int mgb200_graph_get_info(const mgb200_graph *h, mgb200_graph_info *info) {
+  if (!h || !info) return MGB200_ERR_INVALID_ARGUMENT;
+  fill_info(h->g, info);
   return MGB200_OK;
 }
 
@@ -941,6 +965,129 @@ int mgb200_cugraph_pagerank_run(mgb200_graph *h, const mgb200_cugraph_params *pa
   }
   if (stats_out) *stats_out = stats;
   return MGB200_OK;
+}
+
+// ---- HITS (include/mgb200_personalized.h; kernels in hits.cu) ----------------------------------------------------
+
+int mgb200_hits_graph_create_host_u32(int device, uint64_t n, uint64_t m, const uint32_t *from, const uint32_t *to,
+                                      mgb200_hits_graph **out) {
+  if (!out) return MGB200_ERR_INVALID_ARGUMENT;
+  *out = nullptr;
+  if (m > 0 && (!from || !to)) {
+    set_error("null edge arrays");
+    return MGB200_ERR_INVALID_ARGUMENT;
+  }
+  int rc = validate_sizes(n, 0, 1);
+  if (rc) return rc;
+  rc = check_device(device);
+  if (rc) return rc;
+  MGB_CUDA(cudaSetDevice(device));
+  uint32_t *d_from = nullptr, *d_to = nullptr;
+  cudaError_t e;
+  if ((e = cudaMalloc(&d_from, std::max<uint64_t>(m, 1) * sizeof(uint32_t))) != cudaSuccess ||
+      (e = cudaMalloc(&d_to, std::max<uint64_t>(m, 1) * sizeof(uint32_t))) != cudaSuccess) {
+    cudaFree(d_from);
+    return cuda_fail(e, "cudaMalloc(COO)", __FILE__, __LINE__);
+  }
+  const auto t0 = std::chrono::steady_clock::now();
+  rc = upload_coo(device, n, m, from, to, d_from, d_to);
+  const double upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  auto *h = rc ? nullptr : new (std::nothrow) mgb200_hits_graph();
+  if (!rc && !h) {
+    set_error("out of host memory");
+    rc = MGB200_ERR_INVALID_ARGUMENT;
+  }
+  if (!rc) {
+    for (Graph *g : {&h->fwd, &h->rev}) {
+      g->device = device;
+      g->n = n;
+      g->m = m;
+      g->part_rank = 0;
+      g->part_world = 1;
+    }
+    DeviceArrays forward(m, d_from, d_to);
+    rc = build_graph(h->fwd, forward);
+    if (!rc) {
+      DeviceArrays reverse(m, d_to, d_from);  // the same COO, endpoints swapped: rows gather along out-edges
+      rc = build_graph(h->rev, reverse);
+    }
+  }
+  cudaFree(d_from);
+  cudaFree(d_to);
+  if (!rc) {
+    h->fwd.upload_ms = upload_ms;
+    if ((e = cudaMalloc(&h->t_of_f, std::max<uint64_t>(n, 1) * sizeof(uint32_t))) != cudaSuccess ||
+        (e = cudaMalloc(&h->f_of_t, std::max<uint64_t>(n, 1) * sizeof(uint32_t))) != cudaSuccess ||
+        (e = cudaMalloc(&h->scratch, hits_scratch_doubles(n) * sizeof(double))) != cudaSuccess ||
+        (e = cudaMalloc(&h->out_stage, std::max<uint64_t>(2 * n, 1) * sizeof(double))) != cudaSuccess ||
+        (e = cudaEventCreateWithFlags(&h->f_done, cudaEventDisableTiming)) != cudaSuccess ||
+        (e = cudaEventCreateWithFlags(&h->t_done, cudaEventDisableTiming)) != cudaSuccess)
+      rc = cuda_fail(e, "HITS buffers", __FILE__, __LINE__);
+  }
+  if (!rc) rc = hits_permutations(h->fwd, h->rev, h->t_of_f, h->f_of_t);
+  if (rc) {
+    mgb200_hits_graph_destroy(h);
+    return rc;
+  }
+  *out = h;
+  return MGB200_OK;
+}
+
+int mgb200_hits_graph_get_info(const mgb200_hits_graph *h, mgb200_graph_info *forward, mgb200_graph_info *reverse) {
+  if (!h) return MGB200_ERR_INVALID_ARGUMENT;
+  if (forward) fill_info(h->fwd, forward);
+  if (reverse) fill_info(h->rev, reverse);
+  return MGB200_OK;
+}
+
+void mgb200_hits_graph_destroy(mgb200_hits_graph *h) {
+  if (!h) return;
+  cudaSetDevice(h->fwd.device);
+  cudaFree(h->t_of_f);
+  cudaFree(h->f_of_t);
+  cudaFree(h->scratch);
+  cudaFree(h->out_stage);
+  if (h->f_done) cudaEventDestroy(h->f_done);
+  if (h->t_done) cudaEventDestroy(h->t_done);
+  free_graph(h->fwd);
+  free_graph(h->rev);
+  delete h;
+}
+
+int mgb200_hits_run(mgb200_hits_graph *h, const mgb200_hits_params *params, double *hubs_out, double *authorities_out,
+                    mgb200_hits_stats *stats_out) {
+  if (!h || !params) return MGB200_ERR_INVALID_ARGUMENT;
+  const uint64_t n = h->fwd.n;
+  if (n > 0 && (!hubs_out || !authorities_out)) {
+    set_error("hubs_out / authorities_out is null");
+    return MGB200_ERR_INVALID_ARGUMENT;
+  }
+  MGB_CUDA(cudaSetDevice(h->fwd.device));
+  mgb200_hits_stats stats{};
+  int rc = hits_iterate(h->fwd, h->rev, h->t_of_f, h->f_of_t, *params, h->scratch, h->f_done, h->t_done, h->out_stage,
+                        h->out_stage + n, &stats);
+  if (rc) return rc;
+  if (n > 0) {
+    cudaStream_t st = h->fwd.stream;
+    cudaError_t e = cudaMemcpyAsync(hubs_out, h->out_stage, n * sizeof(double), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(authorities_out, h->out_stage + n, n * sizeof(double), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaMemcpyAsync(HITS D2H)", __FILE__, __LINE__);
+  }
+  if (stats_out) *stats_out = stats;
+  return MGB200_OK;
+}
+
+int mgb200_hits(uint64_t n, uint64_t m, const uint32_t *from, const uint32_t *to, const mgb200_hits_params *params,
+                double *hubs_out, double *authorities_out, mgb200_hits_stats *stats) {
+  if (!params) return MGB200_ERR_INVALID_ARGUMENT;
+  const char *dev_env = getenv("MGB200_DEVICE");
+  mgb200_hits_graph *g = nullptr;
+  int rc = mgb200_hits_graph_create_host_u32(dev_env ? atoi(dev_env) : 0, n, m, from, to, &g);
+  if (rc) return rc;
+  rc = mgb200_hits_run(g, params, hubs_out, authorities_out, stats);
+  mgb200_hits_graph_destroy(g);
+  return rc;
 }
 
 int mgb200_partition_range(uint64_t n, uint32_t part_world, uint32_t part_rank, uint64_t *first_label_out,

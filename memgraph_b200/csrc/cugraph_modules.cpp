@@ -1,5 +1,5 @@
-// memgraph_b200/csrc/cugraph_modules.cpp -- stand-ins for the reference's cuGraph PageRank query modules on the GPU
-// compute ABI (include/mgb200_personalized.h).  Compiled twice (memgraph_b200/build.py):
+// memgraph_b200/csrc/cugraph_modules.cpp -- stand-ins for the reference's cuGraph PageRank and HITS query modules on the
+// GPU compute ABI (include/mgb200_personalized.h).  Compiled three times (memgraph_b200/build.py):
 //   -DMGB200_CUGRAPH_PERSONALIZED=0 -> cugraph.pagerank.so               CALL cugraph.pagerank.get(max_iterations = 100,
 //        damping_factor = 0.85, stop_epsilon = 1e-5, weight_property = "weight") YIELD node, pagerank
 //        (mage/cpp/cugraph_module/algorithms/pagerank.cu:60-143)
@@ -7,6 +7,9 @@
 //        personalization_vertices, personalization_values, max_iterations = 100, damping_factor = 0.85,
 //        stop_epsilon = 1e-5, weight_property = "weight") YIELD node, pagerank
 //        (mage/cpp/cugraph_module/algorithms/personalized_pagerank.cu:59-215)
+//   -DMGB200_CUGRAPH_HITS=1         -> cugraph.hits.so                   CALL cugraph.hits.get(max_iterations = 100,
+//        tolerance = 1e-5, normalized = true) YIELD node, hubs, authorities
+//        (mage/cpp/cugraph_module/algorithms/hits.cu: unweighted directed view, no initial hub guess)
 // Same procedure name, argument names / types / defaults / order and result fields.  Behaviour restated from the
 // reference modules: the graph view is weighted (the named edge property when it is a number, else 1.0,
 // include/mg_utils.hpp:166); cuGraph only knows vertices that occur in an edge, so isolated vertices get no row, an isolated
@@ -18,6 +21,7 @@
 #include <cstdint>
 #include <cstdlib>
 #include <exception>
+#include <initializer_list>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -28,6 +32,9 @@
 #ifndef MGB200_CUGRAPH_PERSONALIZED
 #define MGB200_CUGRAPH_PERSONALIZED 0
 #endif
+#ifndef MGB200_CUGRAPH_HITS
+#define MGB200_CUGRAPH_HITS 0
+#endif
 
 using namespace mgb200_module;
 
@@ -36,6 +43,8 @@ namespace {
 constexpr const char *kProcedureGet = "get";
 constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldPageRank = "pagerank";
+constexpr const char *kFieldHubs = "hubs";
+constexpr const char *kFieldAuthorities = "authorities";
 constexpr double kDefaultWeight = 1.0;
 
 struct WeightedView {
@@ -65,6 +74,7 @@ double EdgeWeight(mgp_edge *edge, const char *property, mgp_memory *memory) {
   return kDefaultWeight;
 }
 
+// weight_property == nullptr: an unweighted view (view.weight stays empty)
 WeightedView PullWeightedView(mgp_graph *graph, mgp_memory *memory, const char *weight_property) {
   WeightedView view;
   std::size_t approx_edges = 0;
@@ -72,7 +82,7 @@ WeightedView PullWeightedView(mgp_graph *graph, mgp_memory *memory, const char *
   std::vector<int64_t> from_gid, to_gid, seen;
   from_gid.reserve(approx_edges);
   to_gid.reserve(approx_edges);
-  view.weight.reserve(approx_edges);
+  if (weight_property) view.weight.reserve(approx_edges);
   {
     VerticesIt vertices(graph, memory);
     std::size_t visited = 0;
@@ -88,7 +98,7 @@ WeightedView PullWeightedView(mgp_graph *graph, mgp_memory *memory, const char *
         Check(mgp_vertex_get_id(destination, &destination_id));
         from_gid.push_back(source_id.as_int);
         to_gid.push_back(destination_id.as_int);
-        view.weight.push_back(EdgeWeight(edge, weight_property, memory));
+        if (weight_property) view.weight.push_back(EdgeWeight(edge, weight_property, memory));
       }
       if ((visited & 0xFFF) == 0 && MustAbort(graph)) throw ModuleError("procedure aborted by the host");
     }
@@ -114,13 +124,20 @@ WeightedView PullWeightedView(mgp_graph *graph, mgp_memory *memory, const char *
     if (keep[e]) {
       view.from.push_back(dense_of(from_gid[e]));
       view.to.push_back(dense_of(to_gid[e]));
-      view.weight[kept++] = view.weight[e];
+      if (weight_property) view.weight[kept] = view.weight[e];
+      ++kept;
     }
-  view.weight.resize(kept);
+  if (weight_property) view.weight.resize(kept);
   return view;
 }
 
-void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, double pagerank) {
+struct FloatField {
+  const char *name;
+  double value;
+};
+
+void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid,
+                std::initializer_list<FloatField> fields) {
   mgp_vertex *vertex = nullptr;
   Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
   if (vertex == nullptr) {
@@ -136,13 +153,58 @@ void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_
   if (record == nullptr)
     throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
   Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  OwnedValue value;
-  Check(mgp_value_make_double(pagerank, memory, &value.v));
-  Check(mgp_result_record_insert(record, kFieldPageRank, value.v));
+  for (const FloatField &field : fields) {
+    OwnedValue value;
+    Check(mgp_value_make_double(field.value, memory, &value.v));
+    Check(mgp_result_record_insert(record, field.name, value.v));
+  }
+}
+
+// cugraph.hits.get: the directed view without weights; rows only for vertices in an edge, in ascending gid
+void HitsProcedure(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
+  mgp_value *arg = nullptr;
+  int64_t max_iterations = 0;
+  double tolerance = 0.0;
+  int normalized = 0;
+  Check(mgp_list_at(args, 0, &arg));
+  Check(mgp_value_get_int(arg, &max_iterations));
+  Check(mgp_list_at(args, 1, &arg));
+  Check(mgp_value_get_double(arg, &tolerance));
+  Check(mgp_list_at(args, 2, &arg));
+  Check(mgp_value_get_bool(arg, &normalized));
+
+  const WeightedView view = PullWeightedView(graph, memory, nullptr);
+  const uint64_t n = view.gid_of_dense.size();
+  if (n == 0) return;  // mg_graph->Empty(), or no edges at all: cuGraph has no vertex to score
+
+  mgb200_hits_params params{};
+  params.max_iterations = static_cast<uint64_t>(max_iterations);  // the reference's static_cast<size_t>
+  params.tolerance = tolerance;
+  params.normalized = normalized;
+  std::vector<double> hubs(n), authorities(n);
+  const char *dev_env = std::getenv("MGB200_DEVICE");
+  mgb200_hits_graph *dg = nullptr;
+  if (mgb200_hits_graph_create_host_u32(dev_env ? std::atoi(dev_env) : 0, n, view.from.size(), view.from.data(),
+                                        view.to.data(), &dg) != MGB200_OK)
+    throw ModuleError(mgb200_last_error());
+  mgb200_hits_stats stats{};
+  const int rc = mgb200_hits_run(dg, &params, hubs.data(), authorities.data(), &stats);
+  const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
+  mgb200_hits_graph_destroy(dg);
+  if (rc != MGB200_OK) throw ModuleError(message);
+
+  if (mgp_result_reserve != nullptr) (void)mgp_result_reserve(result, n);
+  for (uint64_t dense = 0; dense < n; ++dense)
+    EmitRecord(graph, result, memory, view.gid_of_dense[dense],
+               {{kFieldHubs, hubs[dense]}, {kFieldAuthorities, authorities[dense]}});
 }
 
 void Procedure(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
   try {
+    if (MGB200_CUGRAPH_HITS) {
+      HitsProcedure(args, graph, result, memory);
+      return;
+    }
     std::size_t next = 0;
     mgp_value *arg = nullptr;
     std::vector<int64_t> seed_gid;
@@ -221,7 +283,8 @@ void Procedure(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory 
     if (rc != MGB200_OK) throw ModuleError(message);
 
     if (mgp_result_reserve != nullptr) (void)mgp_result_reserve(result, n);
-    for (uint64_t dense = 0; dense < n; ++dense) EmitRecord(graph, result, memory, view.gid_of_dense[dense], pageranks[dense]);
+    for (uint64_t dense = 0; dense < n; ++dense)
+      EmitRecord(graph, result, memory, view.gid_of_dense[dense], {{kFieldPageRank, pageranks[dense]}});
   } catch (const std::exception &e) {
     (void)mgp_result_set_error_msg(result, e.what());  // nothing may escape the callback
   } catch (...) {
@@ -238,6 +301,24 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   try {
     mgp_proc *proc = nullptr;
     Check(mgp_module_add_read_procedure(module, kProcedureGet, Procedure, &proc));
+    if (MGB200_CUGRAPH_HITS) {  // registration as in hits.cu's mgp_init_module
+      OwnedValue tolerance, normalized;
+      mgp_type *type_int = nullptr, *type_float = nullptr, *type_bool = nullptr, *type_node = nullptr;
+      Check(mgp_type_int(&type_int));
+      Check(mgp_type_float(&type_float));
+      Check(mgp_type_bool(&type_bool));
+      Check(mgp_type_node(&type_node));
+      Check(mgp_value_make_int(100, memory, &max_iterations.v));
+      Check(mgp_value_make_double(1e-5, memory, &tolerance.v));
+      Check(mgp_value_make_bool(1, memory, &normalized.v));
+      Check(mgp_proc_add_opt_arg(proc, "max_iterations", type_int, max_iterations.v));
+      Check(mgp_proc_add_opt_arg(proc, "tolerance", type_float, tolerance.v));
+      Check(mgp_proc_add_opt_arg(proc, "normalized", type_bool, normalized.v));
+      Check(mgp_proc_add_result(proc, kFieldNode, type_node));
+      Check(mgp_proc_add_result(proc, kFieldHubs, type_float));
+      Check(mgp_proc_add_result(proc, kFieldAuthorities, type_float));
+      return 0;
+    }
     mgp_type *type_int = nullptr, *type_float = nullptr, *type_node = nullptr, *type_string = nullptr;
     Check(mgp_type_int(&type_int));
     Check(mgp_type_float(&type_float));
