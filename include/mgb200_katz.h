@@ -15,7 +15,9 @@
  *   iteration i >= 1:  omega_i[v] = sum_{u -> v} omega_{i-1}[u];  c_i[v] = c_{i-1}[v] + alpha^i omega_i[v]
  *                      lr[v] = c_i[v];  ur[v] = c_i[v] + alpha^(i+1) omega_i[v] gamma
  *   stop when, walking the vertices in std::partial_sort order of c_i descending, no neighbour pair (a, b) has
- *   ur[b] - epsilon >= lr[a].  No edges: every centrality is 0.  The reference has no iteration cap; max_iterations
+ *   ur[b] - epsilon >= lr[a].  ur is computed for EVERY vertex: where omega_i[v] = 0 it is c_i[v] + 0 * gamma, NaN when
+ *   alpha^2 deg_max == 1 makes gamma = +inf, and a NaN bound fails no comparison (so with epsilon <= 0 vertices without
+ *   in-edges do not hold the loop).  No edges: every centrality is 0.  The reference has no iteration cap; max_iterations
  *   below is a guard for callers (0 = none) and reports MGB200_KATZ_NOT_CONVERGED when it ends the loop.
  * Parity: omega_i are walk counts -- integers, exact in FP64 below 2^53 in any summation order -- and every other
  * operation is performed with the reference's association and rounding, so results are BIT-EXACT until a walk count

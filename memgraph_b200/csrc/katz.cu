@@ -7,7 +7,9 @@
 //     ARE the graph handle's two contribution buffers, c lives in its rank array;
 //   * the row epilogue applies c += alpha^i omega, ur = c + alpha^(i+1) omega gamma with the reference's association
 //     and one rounding per operation (no FMA contraction: the reference is compiled for baseline x86-64);
-//   * zero in-degree rows: omega_i = 0 for i >= 1, so c = ur = 0 forever -- set once, never visited;
+//   * zero in-degree rows: omega_i = 0 for i >= 1, so c = 0 and ur = 0 + 0 * gamma forever -- set once, never
+//     visited.  That ur is +0 while gamma is finite and NaN when alpha^2 deg_max == 1 makes gamma = +inf; NaN fails
+//     every comparison, so with epsilon <= 0 these rows still let the test pass, exactly as in the reference;
 //   * the convergence test sorts (c descending) with a radix sort and decides from neighbour pairs.  The reference
 //     sorts with std::partial_sort, which is unstable; the verdict is independent of the order among equal c except
 //     when a group of equal-c vertices contains EXACTLY ONE vertex whose own bound already violates the test against an
@@ -40,15 +42,17 @@ struct Verdict {
   unsigned int max_outdeg;
 };
 
-// context.Init (:33-45): omega_0 = 1, c_0 = 0; omega_1 of the zero in-degree rows is their final value 0
-__global__ void katz_init_kernel(uint64_t n, double *omega0, double *omega1, double *c, double *ur, IterState *state,
-                                 Verdict *verdict) {
+// context.Init (:33-45): omega_0 = 1, c_0 = 0; omega_1 of the zero in-degree rows is their final value 0.  Those rows
+// are never visited again, so their ur is written here once: the reference's c + (alpha^(i+1) * 0) * gamma, which is
+// zero_ur = 0 + 0 * gamma at every iteration -- +0 while gamma is finite, NaN when it is not (alpha^2 deg_max == 1).
+__global__ void katz_init_kernel(uint64_t n, uint64_t zero_lo, uint64_t zero_hi, double zero_ur, double *omega0,
+                                 double *omega1, double *c, double *ur, IterState *state) {
   const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
   for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
     omega0[i] = 1.0;
     omega1[i] = 0.0;
     c[i] = 0.0;
-    ur[i] = 0.0;
+    ur[i] = (i >= zero_lo && i < zero_hi) ? zero_ur : 0.0;
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     omega0[n] = 0.0;  // the slot SELL padding entries read
@@ -56,7 +60,6 @@ __global__ void katz_init_kernel(uint64_t n, double *omega0, double *omega1, dou
     state->done = 0;  // the gather kernels return at once while this is set
     state->error = 0;
     state->iterations = 0ull;
-    verdict->max_outdeg = 0u;
   }
 }
 
@@ -280,18 +283,20 @@ int katz_iterate(Graph &g, double alpha, double epsilon, uint64_t max_iterations
   const int grid_n = blocks_for(n, g.sm_count);
 
   MGB_CUDA(cudaEventRecord(g.ev[2], st));
-  katz_init_kernel<<<grid_n, kThreads, 0, st>>>(n, omega[0], omega[1], c, ur, g.state, verdict);
+  MGB_CUDA(cudaMemsetAsync(verdict, 0, sizeof(Verdict), st));
   max_outdeg_kernel<<<grid_n, kThreads, 0, st>>>(n, g.outdeg_l, verdict);
   Verdict host_verdict{};
   MGB_CUDA(cudaMemcpyAsync(&host_verdict, verdict, sizeof(Verdict), cudaMemcpyDeviceToHost, st));
   MGB_CUDA(cudaStreamSynchronize(st));
-  uint64_t launches = 2;
   const double deg_max = static_cast<double>(host_verdict.max_outdeg);
   const double gamma = deg_max / (1. - (alpha * alpha * deg_max));  // :400
   res->max_out_degree = host_verdict.max_outdeg;
   res->gamma = gamma;
 
   const uint64_t zero_lo = g.zero_lo[0], zero_hi = g.zero_hi[0];  // labels of the zero in-degree rows
+  const double zero_ur = 0.0 + 0.0 * gamma;  // :245 with omega = 0, whatever the sign of alpha^(i+1)
+  katz_init_kernel<<<grid_n, kThreads, 0, st>>>(n, zero_lo, zero_hi, zero_ur, omega[0], omega[1], c, ur, g.state);
+  uint64_t launches = 2;
   uint64_t iteration = 0;
   bool converged = false;
   do {
