@@ -1255,7 +1255,8 @@ int build_graph(Graph &g, EdgeSource &edges) {
     // graph); below that every extra run start costs more than the balance gains and ONE (or two) contiguous runs per
     // warp, dealt statically, are faster (the partitions of a multi-GPU run).
     const uint64_t kSliceCost = env_u32_zero("MGB200_SLICE_COST", 8);
-    const uint64_t resident_warps = static_cast<uint64_t>(g.sm_count) * 32u;  // 4 CTAs x 8 warps per SM
+    const uint64_t resident_warps = static_cast<uint64_t>(g.sm_count) * 32u;  // item basis: 32 warps per SM (the
+                                                                               // kernel holds 3 CTAs x 8 warps)
     const uint64_t per_warp = g.n_slices / resident_warps;
     g.sell_static = g.tun.sell_mode >= 0 ? g.tun.sell_mode == 1 : per_warp < 64;
     const uint64_t items_default = !g.sell_static ? resident_warps * 16 : (per_warp < 32 ? resident_warps : resident_warps * 2);

@@ -405,7 +405,9 @@ struct SellArgs {
 #define MGB_SELL_UNROLL 8      // columns per batch (gathers in flight per lane)
 #endif
 #ifndef MGB_SELL_MIN_BLOCKS
-#define MGB_SELL_MIN_BLOCKS 4  // resident CTAs/SM requested from ptxas (register cap = 65536 / (256 * this))
+#define MGB_SELL_MIN_BLOCKS 3  // resident CTAs/SM requested from ptxas (register cap = 65536 / (256 * this)): at 4 the
+                               // walk is capped at 64 registers and spills 152 bytes; at 3 it takes 80 and spills
+                               // none, 6 % less SELL time despite 24 instead of 32 warps per SM (DESIGN.md §4)
 #endif
 constexpr int kSellUnroll = MGB_SELL_UNROLL;
 
@@ -464,6 +466,13 @@ __device__ __forceinline__ void sell_walk(const SellArgs &a, const double *table
       double v[kSellUnroll];
 #pragma unroll
       for (int j = 0; j < kSellUnroll; ++j) src[j] = nxt[j];
+#ifdef MGB_SELL_HOT_ONLY_FROM  // bound measurement only (wrong ranks): sources >= this label read the zero slot n
+      if (kPath == kPathRange) {
+#pragma unroll
+        for (int j = 0; j < kSellUnroll; ++j)
+          if (src[j] >= MGB_SELL_HOT_ONLY_FROM) src[j] = a.window.total_bytes / sizeof(double) - 1;
+      }
+#endif
 #pragma unroll
       for (int j = 0; j < kSellUnroll; ++j)  // the next batch of indices travels while this batch is gathered
         if (k + kSellUnroll + j < ncols) nxt[j] = ld_index(p + static_cast<size_t>(k + kSellUnroll + j) * kSliceRows, pol);
@@ -530,7 +539,7 @@ __global__ void __launch_bounds__(kBlockThreads, MGB_SELL_MIN_BLOCKS) sell_rows_
   sell_walk<kPathRange, false, true>(a, nullptr);
 }
 
-// The same walk with the hot table: ONE 1024-thread CTA per SM (the same 32 warps as 4 x 256 threads) so that the SM
+// The same walk with the hot table: ONE 1024-thread CTA per SM (32 warps, at most 64 registers each) so that the SM
 // holds one copy of the table; filled once per launch -- one partition: TMA bulk copies (cp.async.bulk, 32 KiB each,
 // completion on an mbarrier, L2 evict-last) of the contiguous label prefix; several partitions: one window per owner,
 // whose first label is only 8-byte aligned, so the threads load it cooperatively.
@@ -1207,7 +1216,7 @@ double zero_row_rank(const Graph &g, const IterateConfig &cfg) {
   return cfg.max_iterations == 0 ? 1.0 / static_cast<double>(g.n) : (1.0 - cfg.damping) / static_cast<double>(g.n);
 }
 
-// SELL rows: the plain kernel (4 x 256 threads per SM) or, with a hot table, one 1024-thread CTA per SM
+// SELL rows: the plain kernel (MGB_SELL_MIN_BLOCKS x 256 threads per SM) or, with a hot table, one 1024-thread CTA per SM
 int launch_sell_rows(Graph &g, const SellArgs &s) {
   const uint32_t table_n = s.window.table_n;
   if (s.w != nullptr) {

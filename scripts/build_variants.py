@@ -14,6 +14,13 @@ VARIANTS = {
     "h_pf5": ["-DMGB_HEAVY_PREFETCH=1", "-DMGB_HEAVY_MIN_BLOCKS=5"], "h_pf4": ["-DMGB_HEAVY_PREFETCH=1", "-DMGB_HEAVY_MIN_BLOCKS=4"],
     "h_b6": ["-DMGB_HEAVY_MIN_BLOCKS=6"], "h_b4": ["-DMGB_HEAVY_MIN_BLOCKS=4"],
     "h_u4pf8": ["-DMGB_HEAVY_PREFETCH=1", "-DMGB_UNROLL=4"], "h_u4b8": ["-DMGB_UNROLL=4"],
+    # bound of a hot-only SELL walk (ranks wrong): every SELL gather from a label >= 2 M (the default block_from) reads
+    # the zero slot instead, so the `sell_rows` class time is the walk without its HBM misses
+    "sell_hot": ["-DMGB_SELL_HOT_ONLY_FROM=2097152"],
+    # SELL walk registers (DESIGN.md §4): 4 CTAs per SM cap it at 64 registers and spill; 3 CTAs do not
+    "s_b4": ["-DMGB_SELL_MIN_BLOCKS=4"], "s_b3": ["-DMGB_SELL_MIN_BLOCKS=3"], "s_u6": ["-DMGB_SELL_UNROLL=6", "-DMGB_SELL_MIN_BLOCKS=4"],
+    "s_u4": ["-DMGB_SELL_UNROLL=4", "-DMGB_SELL_MIN_BLOCKS=4"],
+    "s_u12b3": ["-DMGB_SELL_UNROLL=12", "-DMGB_SELL_MIN_BLOCKS=3"], "s_u16b2": ["-DMGB_SELL_UNROLL=16", "-DMGB_SELL_MIN_BLOCKS=2"],
 }
 
 
@@ -32,11 +39,11 @@ def main():
             raise SystemExit(1)
         sell = ""
         lines = log.stdout.splitlines()
-        for i, l in enumerate(lines):
-            if "Compiling entry function" in l and "heavy_segments_kernelILi0ELb0E" in l:
-                sell = " | ".join(x.strip() for x in lines[i + 1:i + 4])
+        for i, l in enumerate(lines):  # registers and spills of the SELL walk and the heavy-segment kernel
+            if "Compiling entry function" in l and ("sell_rows_kernelILi0E" in l or "heavy_segments_kernelILi0ELb0E" in l):
+                sell += " | ".join(x.strip() for x in lines[i + 2:i + 4]) + "\n           "
         subprocess.run([B.NVCC, "-shared", "-cudart", "static", "-o", os.path.join(out, "libmgb200_pagerank.so"), obj] + others, check=True)
-        print(f"{name:10s} {sell}")
+        print(f"{name:10s} {sell.rstrip()}")
 
 
 if __name__ == "__main__":
