@@ -30,73 +30,36 @@ constexpr const char *kProcedureGet = "get";
 constexpr const char *kArgumentDirected = "directed";
 constexpr const char *kArgumentNormalized = "normalized";
 constexpr const char *kArgumentThreads = "threads";
-constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldBCScore = "betweenness_centrality";
 
-int HostAsksToAbort(void *graph) { return MustAbort(static_cast<mgp_graph *>(graph)) ? 1 : 0; }
-
-void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, double centrality) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return;
-  }
-  OwnedValue node;
-  Check(mgp_value_make_vertex(vertex, &node.v));  // takes ownership of `vertex` on success
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
-  Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  OwnedValue value;
-  Check(mgp_value_make_double(centrality, memory, &value.v));
-  Check(mgp_result_record_insert(record, kFieldBCScore, value.v));
-}
-
 void GetBetweennessCentrality(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    mgp_value *arg = nullptr;
-    int directed = 0, normalized = 0;
-    int64_t threads = 0;
-    Check(mgp_list_at(args, 0, &arg));
-    Check(mgp_value_get_bool(arg, &directed));
-    Check(mgp_list_at(args, 1, &arg));
-    Check(mgp_value_get_bool(arg, &normalized));
-    Check(mgp_list_at(args, 2, &arg));
-    Check(mgp_value_get_int(arg, &threads));
-    (void)threads;
+  mgp_value *arg = nullptr;
+  int directed = 0, normalized = 0;
+  int64_t threads = 0;
+  Check(mgp_list_at(args, 0, &arg));
+  Check(mgp_value_get_bool(arg, &directed));
+  Check(mgp_list_at(args, 1, &arg));
+  Check(mgp_value_get_bool(arg, &normalized));
+  Check(mgp_list_at(args, 2, &arg));
+  Check(mgp_value_get_int(arg, &threads));
+  (void)threads;
 
-    const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped);
-    const uint64_t n = hg.gid_of_dense.size();
-    std::vector<double> bc(n, 0.0);
-    if (n != 0) {  // an empty view yields zero rows in the reference too; nothing to compute anywhere
-      const char *dev_env = std::getenv("MGB200_DEVICE");
-      const std::vector<uint64_t> from64(hg.from.begin(), hg.from.end()), to64(hg.to.begin(), hg.to.end());
-      mgb200_bfs_graph *dg = nullptr;
-      if (mgb200_bfs_graph_create_host(dev_env ? std::atoi(dev_env) : 0, n, from64.size(), from64.data(), to64.data(),
-                                       &dg) != MGB200_OK)
-        throw ModuleError(mgb200_last_error());
-      const int rc = mgb200_bc_run(dg, directed != 0, 0, n, HostAsksToAbort, graph, bc.data(), 0, nullptr);
-      const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-      mgb200_bfs_graph_destroy(dg);
-      if (rc != MGB200_OK) throw ModuleError(message);
-      if (normalized) {  // betweenness_centrality.cpp:138-143; (n - 1) * (n - 2) in uint64_t
-        const uint64_t pairs = (n - 1) * (n - 2);
-        const double constant = n > 2 ? (directed ? 1.0 : 2.0) / static_cast<double>(pairs) : 1.0;
-        for (double &value : bc) value *= constant;
-      }
+  const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped);
+  const uint64_t n = hg.gid_of_dense.size();
+  std::vector<double> bc(n, 0.0);
+  if (n != 0) {  // an empty view yields zero rows in the reference too; nothing to compute anywhere
+    const BfsDeviceGraph dg(hg);
+    CheckDevice(mgb200_bc_run(dg.graph.h, directed != 0, 0, n, MustAbortPoll, graph, bc.data(), 0, nullptr));
+    if (normalized) {  // betweenness_centrality.cpp:138-143; (n - 1) * (n - 2) in uint64_t
+      const uint64_t pairs = (n - 1) * (n - 2);
+      const double constant = n > 2 ? (directed ? 1.0 : 2.0) / static_cast<double>(pairs) : 1.0;
+      for (double &value : bc) value *= constant;
     }
-
-    if (mgp_result_reserve != nullptr && n != 0) (void)mgp_result_reserve(result, n);
-    for (uint64_t dense = 0; dense < n; ++dense) EmitRecord(graph, result, memory, hg.gid_of_dense[dense], bc[dense]);
-  } catch (const std::exception &e) {
-    (void)mgp_result_set_error_msg(result, e.what());  // nothing may escape the callback (reference :61-65)
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
   }
+
+  if (mgp_result_reserve != nullptr && n != 0) (void)mgp_result_reserve(result, n);
+  for (uint64_t dense = 0; dense < n; ++dense)
+    EmitNodeRow(graph, result, memory, hg.gid_of_dense[dense], kFieldBCScore, bc[dense]);
 }
 
 }  // namespace
@@ -107,7 +70,7 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   OwnedValue default_directed, default_normalized, default_threads;  // destroyed on every path (reference :92-102)
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, kProcedureGet, GetBetweennessCentrality, &proc));
+    Check(mgp_module_add_read_procedure(module, kProcedureGet, Guarded<GetBetweennessCentrality>, &proc));
     Check(mgp_value_make_bool(1, memory, &default_directed.v));
     Check(mgp_value_make_bool(1, memory, &default_normalized.v));
     Check(mgp_value_make_int(static_cast<int64_t>(std::thread::hardware_concurrency()), memory, &default_threads.v));

@@ -45,28 +45,11 @@ constexpr const char *kFieldBccId = "bcc_id";
 constexpr const char *kFieldNodeFrom = "node_from";
 constexpr const char *kFieldNodeTo = "node_to";
 
-// The vertex `gid` as a value in *out; false when it has vanished in analytical mode.
-bool NodeValue(mgp_graph *graph, mgp_memory *memory, int64_t gid, OwnedValue *out) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return false;
-  }
-  Check(mgp_value_make_vertex(vertex, &out->v));  // takes ownership of `vertex` on success
-  return true;
-}
-
 void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t from_gid, int64_t to_gid,
                 const int64_t *bcc_id) {
   OwnedValue from, to;
   if (!NodeValue(graph, memory, from_gid, &from) || !NodeValue(graph, memory, to_gid, &to)) return;
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
+  mgp_result_record *record = NewRecord(result);
   if (bcc_id) {
     OwnedValue value;
     Check(mgp_value_make_int(*bcc_id, memory, &value.v));
@@ -77,48 +60,35 @@ void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_
 }
 
 void Get(mgp_list * /*args*/, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped);
-    const uint64_t n = hg.gid_of_dense.size(), m = hg.from.size();
-    if (n == 0) return;
-    std::vector<uint8_t> bridge(m, 0);
-    std::vector<int64_t> bcc(m, -1);
-    {
-      const char *dev_env = std::getenv("MGB200_DEVICE");
-      const std::vector<uint64_t> from64(hg.from.begin(), hg.from.end()), to64(hg.to.begin(), hg.to.end());
-      mgb200_bfs_graph *dg = nullptr;
-      if (mgb200_bfs_graph_create_host(dev_env ? std::atoi(dev_env) : 0, n, m, from64.data(), to64.data(), &dg) !=
-          MGB200_OK)
-        throw ModuleError(mgb200_last_error());
-      const int rc = mgb200_biconnectivity_run(dg, m, from64.data(), to64.data(), MGB200_BRIDGES ? bridge.data() : nullptr,
-                                               MGB200_BRIDGES ? nullptr : bcc.data(), nullptr);
-      const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-      mgb200_bfs_graph_destroy(dg);
-      if (rc != MGB200_OK) throw ModuleError(message);
-    }
-#if MGB200_BRIDGES
-    for (uint64_t e = 0; e < m; ++e)
-      if (bridge[e]) EmitRecord(graph, result, memory, hg.gid_of_dense[hg.from[e]], hg.gid_of_dense[hg.to[e]], nullptr);
-#else
-    // a stable counting sort of the non-loop edges by component: ascending bcc_id, view edge order inside
-    int64_t components = 0;
-    for (uint64_t e = 0; e < m; ++e) components = std::max(components, bcc[e] + 1);
-    std::vector<uint64_t> start(components + 1, 0);
-    for (uint64_t e = 0; e < m; ++e)
-      if (bcc[e] >= 0) ++start[bcc[e] + 1];
-    for (int64_t c = 0; c < components; ++c) start[c + 1] += start[c];
-    std::vector<uint64_t> rows(start[components]);
-    for (uint64_t e = 0; e < m; ++e)
-      if (bcc[e] >= 0) rows[start[bcc[e]]++] = e;
-    if (mgp_result_reserve != nullptr && !rows.empty()) (void)mgp_result_reserve(result, rows.size());
-    for (const uint64_t e : rows)
-      EmitRecord(graph, result, memory, hg.gid_of_dense[hg.from[e]], hg.gid_of_dense[hg.to[e]], &bcc[e]);
-#endif
-  } catch (const std::exception &e) {
-    (void)mgp_result_set_error_msg(result, e.what());  // nothing may escape the callback
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
+  const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped);
+  const uint64_t n = hg.gid_of_dense.size(), m = hg.from.size();
+  if (n == 0) return;
+  std::vector<uint8_t> bridge(m, 0);
+  std::vector<int64_t> bcc(m, -1);
+  {
+    const BfsDeviceGraph dg(hg);
+    CheckDevice(mgb200_biconnectivity_run(dg.graph.h, m, dg.from.data(), dg.to.data(),
+                                          MGB200_BRIDGES ? bridge.data() : nullptr, MGB200_BRIDGES ? nullptr : bcc.data(),
+                                          nullptr));
   }
+#if MGB200_BRIDGES
+  for (uint64_t e = 0; e < m; ++e)
+    if (bridge[e]) EmitRecord(graph, result, memory, hg.gid_of_dense[hg.from[e]], hg.gid_of_dense[hg.to[e]], nullptr);
+#else
+  // a stable counting sort of the non-loop edges by component: ascending bcc_id, view edge order inside
+  int64_t components = 0;
+  for (uint64_t e = 0; e < m; ++e) components = std::max(components, bcc[e] + 1);
+  std::vector<uint64_t> start(components + 1, 0);
+  for (uint64_t e = 0; e < m; ++e)
+    if (bcc[e] >= 0) ++start[bcc[e] + 1];
+  for (int64_t c = 0; c < components; ++c) start[c + 1] += start[c];
+  std::vector<uint64_t> rows(start[components]);
+  for (uint64_t e = 0; e < m; ++e)
+    if (bcc[e] >= 0) rows[start[bcc[e]]++] = e;
+  if (mgp_result_reserve != nullptr && !rows.empty()) (void)mgp_result_reserve(result, rows.size());
+  for (const uint64_t e : rows)
+    EmitRecord(graph, result, memory, hg.gid_of_dense[hg.from[e]], hg.gid_of_dense[hg.to[e]], &bcc[e]);
+#endif
 }
 
 }  // namespace
@@ -128,7 +98,7 @@ extern "C" {
 __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *module, struct mgp_memory * /*memory*/) {
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, kProcedureGet, Get, &proc));
+    Check(mgp_module_add_read_procedure(module, kProcedureGet, Guarded<Get>, &proc));
     mgp_type *type_node = nullptr;
     Check(mgp_type_node(&type_node));
     if (!MGB200_BRIDGES) {

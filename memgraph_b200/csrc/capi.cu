@@ -30,6 +30,12 @@ namespace mgb200 {
 
 namespace {
 thread_local std::string tls_error;
+
+// The device the one-shot entry points run on: MGB200_DEVICE, default 0.
+int device_from_env() {
+  const char *dev_env = getenv("MGB200_DEVICE");
+  return dev_env ? atoi(dev_env) : 0;
+}
 }
 
 void set_error(const std::string &msg) { tls_error = msg; }
@@ -737,8 +743,7 @@ int mgb200_parallel_iterative_pagerank(uint64_t n, uint64_t m, const uint64_t *f
     }
     return MGB200_OK;
   }
-  const char *dev_env = getenv("MGB200_DEVICE");
-  const int device = dev_env ? atoi(dev_env) : 0;
+  const int device = device_from_env();
   mgb200_graph *g = nullptr;
   int rc = mgb200_graph_create_host(device, n, m, from, to, 0, 1, &g);
   if (rc) return rc;
@@ -780,8 +785,7 @@ int pagerank_multi_impl(uint64_t n, uint64_t m, const T *from, const T *to, cons
     if (n == 0)
       return mgb200_parallel_iterative_pagerank(n, 0, nullptr, nullptr, params->max_iterations, params->damping_factor,
                                                 params->stop_epsilon, number_of_threads, rank_out, iterations_out);
-    const char *dev_env = getenv("MGB200_DEVICE");
-    const int device = devices ? devices[0] : (dev_env ? atoi(dev_env) : 0);
+    const int device = devices ? devices[0] : device_from_env();
     mgb200_graph *g = nullptr;
     int rc = create_from_host(device, n, m, from, to, 0, 1, &g);
     if (rc) return rc;
@@ -923,10 +927,8 @@ int mgb200_katz_run(mgb200_graph *h, double alpha, double epsilon, uint64_t max_
 
 int mgb200_katz_centrality(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to, double alpha,
                            double epsilon, uint64_t max_iterations, double *centrality_out, uint64_t *iterations_out) {
-  const char *dev_env = getenv("MGB200_DEVICE");
-  const int device = dev_env ? atoi(dev_env) : 0;
   mgb200_graph *g = nullptr;
-  int rc = mgb200_graph_create_host(device, n, m, from, to, 0, 1, &g);  // fails without a device, also for n == 0
+  int rc = mgb200_graph_create_host(device_from_env(), n, m, from, to, 0, 1, &g);  // fails without a device, also for n == 0
   if (rc) return rc;
   mgb200_katz_stats stats{};
   rc = mgb200_katz_run(g, alpha, epsilon, max_iterations, centrality_out, &stats);
@@ -1081,9 +1083,8 @@ int mgb200_hits_run(mgb200_hits_graph *h, const mgb200_hits_params *params, doub
 int mgb200_hits(uint64_t n, uint64_t m, const uint32_t *from, const uint32_t *to, const mgb200_hits_params *params,
                 double *hubs_out, double *authorities_out, mgb200_hits_stats *stats) {
   if (!params) return MGB200_ERR_INVALID_ARGUMENT;
-  const char *dev_env = getenv("MGB200_DEVICE");
   mgb200_hits_graph *g = nullptr;
-  int rc = mgb200_hits_graph_create_host_u32(dev_env ? atoi(dev_env) : 0, n, m, from, to, &g);
+  int rc = mgb200_hits_graph_create_host_u32(device_from_env(), n, m, from, to, &g);
   if (rc) return rc;
   rc = mgb200_hits_run(g, params, hubs_out, authorities_out, stats);
   mgb200_hits_graph_destroy(g);

@@ -21,7 +21,6 @@
 #include <cstdint>
 #include <cstdlib>
 #include <exception>
-#include <initializer_list>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -41,7 +40,6 @@ using namespace mgb200_module;
 namespace {
 
 constexpr const char *kProcedureGet = "get";
-constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldPageRank = "pagerank";
 constexpr const char *kFieldHubs = "hubs";
 constexpr const char *kFieldAuthorities = "authorities";
@@ -131,35 +129,6 @@ WeightedView PullWeightedView(mgp_graph *graph, mgp_memory *memory, const char *
   return view;
 }
 
-struct FloatField {
-  const char *name;
-  double value;
-};
-
-void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid,
-                std::initializer_list<FloatField> fields) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return;
-  }
-  OwnedValue node;
-  Check(mgp_value_make_vertex(vertex, &node.v));  // takes ownership of `vertex` on success
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
-  Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  for (const FloatField &field : fields) {
-    OwnedValue value;
-    Check(mgp_value_make_double(field.value, memory, &value.v));
-    Check(mgp_result_record_insert(record, field.name, value.v));
-  }
-}
-
 // cugraph.hits.get: the directed view without weights; rows only for vertices in an edge, in ascending gid
 void HitsProcedure(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
   mgp_value *arg = nullptr;
@@ -182,114 +151,102 @@ void HitsProcedure(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_mem
   params.tolerance = tolerance;
   params.normalized = normalized;
   std::vector<double> hubs(n), authorities(n);
-  const char *dev_env = std::getenv("MGB200_DEVICE");
-  mgb200_hits_graph *dg = nullptr;
-  if (mgb200_hits_graph_create_host_u32(dev_env ? std::atoi(dev_env) : 0, n, view.from.size(), view.from.data(),
-                                        view.to.data(), &dg) != MGB200_OK)
-    throw ModuleError(mgb200_last_error());
-  mgb200_hits_stats stats{};
-  const int rc = mgb200_hits_run(dg, &params, hubs.data(), authorities.data(), &stats);
-  const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-  mgb200_hits_graph_destroy(dg);
-  if (rc != MGB200_OK) throw ModuleError(message);
+  {
+    HitsGraph dg;
+    CheckDevice(mgb200_hits_graph_create_host_u32(DeviceFromEnv(), n, view.from.size(), view.from.data(), view.to.data(),
+                                                  &dg.h));
+    mgb200_hits_stats stats{};
+    CheckDevice(mgb200_hits_run(dg.h, &params, hubs.data(), authorities.data(), &stats));
+  }
 
   if (mgp_result_reserve != nullptr) (void)mgp_result_reserve(result, n);
   for (uint64_t dense = 0; dense < n; ++dense)
-    EmitRecord(graph, result, memory, view.gid_of_dense[dense],
-               {{kFieldHubs, hubs[dense]}, {kFieldAuthorities, authorities[dense]}});
+    EmitNodeRow(graph, result, memory, view.gid_of_dense[dense], kFieldHubs, hubs[dense], kFieldAuthorities,
+                authorities[dense]);
 }
 
 void Procedure(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    if (MGB200_CUGRAPH_HITS) {
-      HitsProcedure(args, graph, result, memory);
-      return;
-    }
-    std::size_t next = 0;
-    mgp_value *arg = nullptr;
-    std::vector<int64_t> seed_gid;
-    std::vector<double> seed_value;
-    if (MGB200_CUGRAPH_PERSONALIZED) {
-      mgp_list *vertices = nullptr, *values = nullptr;
-      Check(mgp_list_at(args, next++, &arg));
-      Check(mgp_value_get_list(arg, &vertices));
-      Check(mgp_list_at(args, next++, &arg));
-      Check(mgp_value_get_list(arg, &values));
-      std::size_t n_seeds = 0, n_values = 0;
-      Check(mgp_list_size(vertices, &n_seeds));
-      Check(mgp_list_size(values, &n_values));
-      if (n_seeds != n_values)
-        throw ModuleError("personalization_vertices and personalization_values must have the same length.");
-      if (n_seeds == 0) return;
-      for (std::size_t i = 0; i < n_seeds; ++i) {
-        mgp_value *item = nullptr;
-        mgp_vertex *vertex = nullptr;
-        Check(mgp_list_at(vertices, i, &item));
-        Check(mgp_value_get_vertex(item, &vertex));
-        mgp_vertex_id id{};
-        Check(mgp_vertex_get_id(vertex, &id));
-        double value = 0.0;
-        Check(mgp_list_at(values, i, &item));
-        Check(mgp_value_get_double(item, &value));
-        seed_gid.push_back(id.as_int);
-        seed_value.push_back(value);
-      }
-    }
-    int64_t max_iterations = 0;
-    double damping_factor = 0.0, stop_epsilon = 0.0;
-    const char *weight_property = nullptr;
-    Check(mgp_list_at(args, next++, &arg));
-    Check(mgp_value_get_int(arg, &max_iterations));
-    Check(mgp_list_at(args, next++, &arg));
-    Check(mgp_value_get_double(arg, &damping_factor));
-    Check(mgp_list_at(args, next++, &arg));
-    Check(mgp_value_get_double(arg, &stop_epsilon));
-    Check(mgp_list_at(args, next++, &arg));
-    Check(mgp_value_get_string(arg, &weight_property));
-
-    const WeightedView view = PullWeightedView(graph, memory, weight_property);
-    const uint64_t n = view.gid_of_dense.size();
-    if (n == 0) return;  // mg_graph->Empty(), or no edges at all: cuGraph has no vertex to rank
-
-    std::vector<uint64_t> seeds;
-    std::vector<double> values;
-    if (MGB200_CUGRAPH_PERSONALIZED) {
-      for (std::size_t i = 0; i < seed_gid.size(); ++i) {
-        const auto it = std::lower_bound(view.gid_of_dense.begin(), view.gid_of_dense.end(), seed_gid[i]);
-        if (it == view.gid_of_dense.end() || *it != seed_gid[i]) continue;  // isolated seed: skipped (:116-119)
-        seeds.push_back(static_cast<uint64_t>(it - view.gid_of_dense.begin()));
-        values.push_back(seed_value[i]);
-      }
-      if (seeds.empty()) return;  // :123
-    }
-
-    const char *dev_env = std::getenv("MGB200_DEVICE");
-    mgb200_graph *dg = nullptr;
-    if (mgb200_graph_create_host_weighted_u32(dev_env ? std::atoi(dev_env) : 0, n, view.from.size(), view.from.data(),
-                                              view.to.data(), view.weight.data(), &dg) != MGB200_OK)
-      throw ModuleError(mgb200_last_error());
-    mgb200_cugraph_params params{};
-    params.max_iterations = static_cast<uint64_t>(max_iterations);
-    params.damping_factor = damping_factor;
-    params.stop_epsilon = stop_epsilon;
-    params.n_personalization = seeds.size();
-    params.personalization_vertices = seeds.data();
-    params.personalization_values = values.data();
-    std::vector<double> pageranks(n);
-    mgb200_cugraph_stats stats{};
-    const int rc = mgb200_cugraph_pagerank_run(dg, &params, pageranks.data(), &stats);
-    const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-    mgb200_graph_destroy(dg);
-    if (rc != MGB200_OK) throw ModuleError(message);
-
-    if (mgp_result_reserve != nullptr) (void)mgp_result_reserve(result, n);
-    for (uint64_t dense = 0; dense < n; ++dense)
-      EmitRecord(graph, result, memory, view.gid_of_dense[dense], {{kFieldPageRank, pageranks[dense]}});
-  } catch (const std::exception &e) {
-    (void)mgp_result_set_error_msg(result, e.what());  // nothing may escape the callback
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
+  if (MGB200_CUGRAPH_HITS) {
+    HitsProcedure(args, graph, result, memory);
+    return;
   }
+  std::size_t next = 0;
+  mgp_value *arg = nullptr;
+  std::vector<int64_t> seed_gid;
+  std::vector<double> seed_value;
+  if (MGB200_CUGRAPH_PERSONALIZED) {
+    mgp_list *vertices = nullptr, *values = nullptr;
+    Check(mgp_list_at(args, next++, &arg));
+    Check(mgp_value_get_list(arg, &vertices));
+    Check(mgp_list_at(args, next++, &arg));
+    Check(mgp_value_get_list(arg, &values));
+    std::size_t n_seeds = 0, n_values = 0;
+    Check(mgp_list_size(vertices, &n_seeds));
+    Check(mgp_list_size(values, &n_values));
+    if (n_seeds != n_values)
+      throw ModuleError("personalization_vertices and personalization_values must have the same length.");
+    if (n_seeds == 0) return;
+    for (std::size_t i = 0; i < n_seeds; ++i) {
+      mgp_value *item = nullptr;
+      mgp_vertex *vertex = nullptr;
+      Check(mgp_list_at(vertices, i, &item));
+      Check(mgp_value_get_vertex(item, &vertex));
+      mgp_vertex_id id{};
+      Check(mgp_vertex_get_id(vertex, &id));
+      double value = 0.0;
+      Check(mgp_list_at(values, i, &item));
+      Check(mgp_value_get_double(item, &value));
+      seed_gid.push_back(id.as_int);
+      seed_value.push_back(value);
+    }
+  }
+  int64_t max_iterations = 0;
+  double damping_factor = 0.0, stop_epsilon = 0.0;
+  const char *weight_property = nullptr;
+  Check(mgp_list_at(args, next++, &arg));
+  Check(mgp_value_get_int(arg, &max_iterations));
+  Check(mgp_list_at(args, next++, &arg));
+  Check(mgp_value_get_double(arg, &damping_factor));
+  Check(mgp_list_at(args, next++, &arg));
+  Check(mgp_value_get_double(arg, &stop_epsilon));
+  Check(mgp_list_at(args, next++, &arg));
+  Check(mgp_value_get_string(arg, &weight_property));
+
+  const WeightedView view = PullWeightedView(graph, memory, weight_property);
+  const uint64_t n = view.gid_of_dense.size();
+  if (n == 0) return;  // mg_graph->Empty(), or no edges at all: cuGraph has no vertex to rank
+
+  std::vector<uint64_t> seeds;
+  std::vector<double> values;
+  if (MGB200_CUGRAPH_PERSONALIZED) {
+    for (std::size_t i = 0; i < seed_gid.size(); ++i) {
+      const auto it = std::lower_bound(view.gid_of_dense.begin(), view.gid_of_dense.end(), seed_gid[i]);
+      if (it == view.gid_of_dense.end() || *it != seed_gid[i]) continue;  // isolated seed: skipped (:116-119)
+      seeds.push_back(static_cast<uint64_t>(it - view.gid_of_dense.begin()));
+      values.push_back(seed_value[i]);
+    }
+    if (seeds.empty()) return;  // :123
+  }
+
+  mgb200_cugraph_params params{};
+  params.max_iterations = static_cast<uint64_t>(max_iterations);
+  params.damping_factor = damping_factor;
+  params.stop_epsilon = stop_epsilon;
+  params.n_personalization = seeds.size();
+  params.personalization_vertices = seeds.data();
+  params.personalization_values = values.data();
+  std::vector<double> pageranks(n);
+  {
+    DeviceGraph dg;
+    CheckDevice(mgb200_graph_create_host_weighted_u32(DeviceFromEnv(), n, view.from.size(), view.from.data(),
+                                                      view.to.data(), view.weight.data(), &dg.h));
+    mgb200_cugraph_stats stats{};
+    CheckDevice(mgb200_cugraph_pagerank_run(dg.h, &params, pageranks.data(), &stats));
+  }
+
+  if (mgp_result_reserve != nullptr) (void)mgp_result_reserve(result, n);
+  for (uint64_t dense = 0; dense < n; ++dense)
+    EmitNodeRow(graph, result, memory, view.gid_of_dense[dense], kFieldPageRank, pageranks[dense]);
 }
 
 }  // namespace
@@ -300,7 +257,7 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   OwnedValue max_iterations, damping_factor, stop_epsilon, weight_property;
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, kProcedureGet, Procedure, &proc));
+    Check(mgp_module_add_read_procedure(module, kProcedureGet, Guarded<Procedure>, &proc));
     if (MGB200_CUGRAPH_HITS) {  // registration as in hits.cu's mgp_init_module
       OwnedValue tolerance, normalized;
       mgp_type *type_int = nullptr, *type_float = nullptr, *type_bool = nullptr, *type_node = nullptr;

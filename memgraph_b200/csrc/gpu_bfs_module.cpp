@@ -24,76 +24,43 @@ using namespace mgb200_module;
 
 namespace {
 
-constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldDistance = "distance";
 
-void EmitDistance(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, int64_t distance) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return;
-  }
-  OwnedValue node;
-  Check(mgp_value_make_vertex(vertex, &node.v));
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
-  Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  OwnedValue value;
-  Check(mgp_value_make_int(distance, memory, &value.v));
-  Check(mgp_result_record_insert(record, kFieldDistance, value.v));
-}
-
 void Distances(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    mgp_value *arg = nullptr;
-    mgp_vertex *source = nullptr;
-    int64_t direction = 0, lower = 1, upper = -1;
-    Check(mgp_list_at(args, 0, &arg));
-    Check(mgp_value_get_vertex(arg, &source));
-    Check(mgp_list_at(args, 1, &arg));
-    Check(mgp_value_get_int(arg, &direction));
-    Check(mgp_list_at(args, 2, &arg));
-    Check(mgp_value_get_int(arg, &lower));
-    Check(mgp_list_at(args, 3, &arg));
-    Check(mgp_value_get_int(arg, &upper));
-    if (direction < MGB200_BFS_OUT || direction > MGB200_BFS_BOTH)
-      throw ModuleError("direction must be 0 (OUT), 1 (IN) or 2 (BOTH)");
-    if (upper < 0) upper = std::numeric_limits<int64_t>::max();
-    mgp_vertex_id source_id{};
-    Check(mgp_vertex_get_id(source, &source_id));
+  mgp_value *arg = nullptr;
+  mgp_vertex *source = nullptr;
+  int64_t direction = 0, lower = 1, upper = -1;
+  Check(mgp_list_at(args, 0, &arg));
+  Check(mgp_value_get_vertex(arg, &source));
+  Check(mgp_list_at(args, 1, &arg));
+  Check(mgp_value_get_int(arg, &direction));
+  Check(mgp_list_at(args, 2, &arg));
+  Check(mgp_value_get_int(arg, &lower));
+  Check(mgp_list_at(args, 3, &arg));
+  Check(mgp_value_get_int(arg, &upper));
+  if (direction < MGB200_BFS_OUT || direction > MGB200_BFS_BOTH)
+    throw ModuleError("direction must be 0 (OUT), 1 (IN) or 2 (BOTH)");
+  if (upper < 0) upper = std::numeric_limits<int64_t>::max();
+  mgp_vertex_id source_id{};
+  Check(mgp_vertex_get_id(source, &source_id));
 
-    // an edge to a vertex the iterator never showed is dropped here: the reference cursor has no "map it to the first
-    // vertex" behaviour (that is a PageRank-module quirk), and a fabricated edge would change distances
-    const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped);
-    const uint64_t n = hg.gid_of_dense.size();
-    uint64_t source_dense = n;
-    if (!hg.dense_of_gid.Find(source_id.as_int, &source_dense)) throw ModuleError("Invalid ID!");
+  // an edge to a vertex the iterator never showed is dropped here: the reference cursor has no "map it to the first
+  // vertex" behaviour (that is a PageRank-module quirk), and a fabricated edge would change distances
+  const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped);
+  const uint64_t n = hg.gid_of_dense.size();
+  uint64_t source_dense = n;
+  if (!hg.dense_of_gid.Find(source_id.as_int, &source_dense)) throw ModuleError("Invalid ID!");
 
-    const char *dev_env = std::getenv("MGB200_DEVICE");
-    mgb200_bfs_graph *dg = nullptr;
-    const std::vector<uint64_t> from64(hg.from.begin(), hg.from.end()), to64(hg.to.begin(), hg.to.end());
-    if (mgb200_bfs_graph_create_host(dev_env ? std::atoi(dev_env) : 0, n, from64.size(), from64.data(), to64.data(),
-                                     &dg) != MGB200_OK)
-      throw ModuleError(mgb200_last_error());
-    std::vector<int32_t> dist(n);
+  std::vector<int32_t> dist(n);
+  {
+    const BfsDeviceGraph dg(hg);
     mgb200_bfs_stats stats{};
-    const int rc = mgb200_bfs_run(dg, source_dense, static_cast<int>(direction), lower, upper, dist.data(), 0, &stats);
-    const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-    mgb200_bfs_graph_destroy(dg);
-    if (rc != MGB200_OK) throw ModuleError(message);
-
-    for (uint64_t v = 0; v < n; ++v)
-      if (dist[v] >= 0) EmitDistance(graph, result, memory, hg.gid_of_dense[v], dist[v]);
-  } catch (const std::exception &e) {
-    (void)mgp_result_set_error_msg(result, e.what());
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
+    CheckDevice(mgb200_bfs_run(dg.graph.h, source_dense, static_cast<int>(direction), lower, upper, dist.data(), 0,
+                               &stats));
   }
+
+  for (uint64_t v = 0; v < n; ++v)
+    if (dist[v] >= 0) EmitNodeRow(graph, result, memory, hg.gid_of_dense[v], kFieldDistance, dist[v]);
 }
 
 }  // namespace
@@ -104,7 +71,7 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   OwnedValue direction, lower, upper;
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, "distances", Distances, &proc));
+    Check(mgp_module_add_read_procedure(module, "distances", Guarded<Distances>, &proc));
     mgp_type *type_int = nullptr, *type_node = nullptr;
     Check(mgp_type_int(&type_int));
     Check(mgp_type_node(&type_node));

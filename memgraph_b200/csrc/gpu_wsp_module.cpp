@@ -47,7 +47,6 @@ using namespace mgb200_module;
 
 namespace {
 
-constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldTotalWeight = "total_weight";
 constexpr const char *kFieldHops = "hops";
 constexpr int64_t kUnbounded = std::numeric_limits<int64_t>::max();
@@ -153,87 +152,52 @@ struct ReadWeight {
   }
 };
 
-void Emit(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, double total, int64_t hops) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return;
-  }
-  OwnedValue node;
-  Check(mgp_value_make_vertex(vertex, &node.v));
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
-  Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  OwnedValue total_value, hops_value;
-  Check(mgp_value_make_double(total, memory, &total_value.v));
-  Check(mgp_result_record_insert(record, kFieldTotalWeight, total_value.v));
-  Check(mgp_value_make_int(hops, memory, &hops_value.v));
-  Check(mgp_result_record_insert(record, kFieldHops, hops_value.v));
-}
-
-int AbortPoll(void *graph) { return MustAbort(static_cast<mgp_graph *>(graph)) ? 1 : 0; }
-
 void Distances(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    mgp_value *arg = nullptr;
-    mgp_vertex *source = nullptr;
-    const char *property = nullptr;
-    int64_t direction = 0, upper = -1;
-    Check(mgp_list_at(args, 0, &arg));
-    Check(mgp_value_get_vertex(arg, &source));
-    Check(mgp_list_at(args, 1, &arg));
-    Check(mgp_value_get_string(arg, &property));
-    Check(mgp_list_at(args, 2, &arg));
-    Check(mgp_value_get_int(arg, &direction));
-    Check(mgp_list_at(args, 3, &arg));
-    Check(mgp_value_get_int(arg, &upper));
-    if (direction < MGB200_BFS_OUT || direction > MGB200_BFS_BOTH)
-      throw ModuleError("direction must be 0 (OUT), 1 (IN) or 2 (BOTH)");
-    if (upper == -1) upper = kUnbounded;
-    if (upper < 1) throw ModuleError("Maximum depth in weighted shortest path expansion must be at least 1.");
-    mgp_vertex_id source_id{};
-    Check(mgp_vertex_get_id(source, &source_id));
+  mgp_value *arg = nullptr;
+  mgp_vertex *source = nullptr;
+  const char *property = nullptr;
+  int64_t direction = 0, upper = -1;
+  Check(mgp_list_at(args, 0, &arg));
+  Check(mgp_value_get_vertex(arg, &source));
+  Check(mgp_list_at(args, 1, &arg));
+  Check(mgp_value_get_string(arg, &property));
+  Check(mgp_list_at(args, 2, &arg));
+  Check(mgp_value_get_int(arg, &direction));
+  Check(mgp_list_at(args, 3, &arg));
+  Check(mgp_value_get_int(arg, &upper));
+  if (direction < MGB200_BFS_OUT || direction > MGB200_BFS_BOTH)
+    throw ModuleError("direction must be 0 (OUT), 1 (IN) or 2 (BOTH)");
+  if (upper == -1) upper = kUnbounded;
+  if (upper < 1) throw ModuleError("Maximum depth in weighted shortest path expansion must be at least 1.");
+  mgp_vertex_id source_id{};
+  Check(mgp_vertex_get_id(source, &source_id));
 
-    // edges to vertices the iterator never showed are dropped, as gpu_bfs does: a fabricated edge would change totals
-    std::vector<EdgeWeight> weights;
-    const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped, ReadWeight{property, memory}, &weights);
-    const uint64_t n = hg.gid_of_dense.size(), m = hg.from.size();
-    uint64_t source_dense = n;
-    if (!hg.dense_of_gid.Find(source_id.as_int, &source_dense)) throw ModuleError("Invalid ID!");
+  // edges to vertices the iterator never showed are dropped, as gpu_bfs does: a fabricated edge would change totals
+  std::vector<EdgeWeight> weights;
+  const HostGraph hg = PullGraph(graph, memory, UnknownGid::kUnknownDropped, ReadWeight{property, memory}, &weights);
+  const uint64_t n = hg.gid_of_dense.size(), m = hg.from.size();
+  uint64_t source_dense = n;
+  if (!hg.dense_of_gid.Find(source_id.as_int, &source_dense)) throw ModuleError("Invalid ID!");
 
-    const std::vector<uint64_t> from64(hg.from.begin(), hg.from.end()), to64(hg.to.begin(), hg.to.end());
-    std::vector<double> w(m);
-    for (uint64_t e = 0; e < m; ++e)
-      w[e] = weights[e].kind == EdgeWeight::kNumber ? weights[e].value : std::numeric_limits<double>::quiet_NaN();
-    const char *dev_env = std::getenv("MGB200_DEVICE");
-    mgb200_bfs_graph *dg = nullptr;
-    if (mgb200_bfs_graph_create_host(dev_env ? std::atoi(dev_env) : 0, n, m, from64.data(), to64.data(), &dg) !=
-        MGB200_OK)
-      throw ModuleError(mgb200_last_error());
-    std::vector<double> dist(n);
-    std::vector<int32_t> hops(n);
+  std::vector<double> w(m);
+  for (uint64_t e = 0; e < m; ++e)
+    w[e] = weights[e].kind == EdgeWeight::kNumber ? weights[e].value : std::numeric_limits<double>::quiet_NaN();
+  std::vector<double> dist(n);
+  std::vector<int32_t> hops(n);
+  {
+    const BfsDeviceGraph dg(hg);
     mgb200_wsp_stats stats{};
-    int rc = mgb200_bfs_graph_set_weights(dg, m, from64.data(), to64.data(), w.data());
+    int rc = mgb200_bfs_graph_set_weights(dg.graph.h, m, dg.from.data(), dg.to.data(), w.data());
     if (rc == MGB200_OK)
-      rc = mgb200_wsp_run(dg, source_dense, static_cast<int>(direction), upper, AbortPoll, graph, dist.data(),
-                          hops.data(), &stats);
-    const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-    mgb200_bfs_graph_destroy(dg);
+      rc = mgb200_wsp_run(dg.graph.h, source_dense, static_cast<int>(direction), upper, MustAbortPoll, graph,
+                          dist.data(), hops.data(), &stats);
     if (rc == MGB200_ERR_INVALID_WEIGHT) throw ModuleError(WeightError(weights[stats.invalid_edge]));
-    if (rc != MGB200_OK) throw ModuleError(message);
-
-    for (uint64_t v = 0; v < n; ++v)
-      if (hops[v] >= 0) Emit(graph, result, memory, hg.gid_of_dense[v], dist[v], hops[v]);
-  } catch (const std::exception &e) {
-    (void)mgp_result_set_error_msg(result, e.what());
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
+    CheckDevice(rc);
   }
+
+  for (uint64_t v = 0; v < n; ++v)
+    if (hops[v] >= 0)
+      EmitNodeRow(graph, result, memory, hg.gid_of_dense[v], kFieldTotalWeight, dist[v], kFieldHops, hops[v]);
 }
 
 }  // namespace
@@ -244,7 +208,7 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   OwnedValue weight_property, direction, upper;
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, "distances", Distances, &proc));
+    Check(mgp_module_add_read_procedure(module, "distances", Guarded<Distances>, &proc));
     mgp_type *type_int = nullptr, *type_float = nullptr, *type_node = nullptr, *type_string = nullptr;
     Check(mgp_type_int(&type_int));
     Check(mgp_type_float(&type_float));

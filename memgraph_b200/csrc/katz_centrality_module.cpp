@@ -29,7 +29,6 @@ namespace {
 constexpr const char *kProcedureGet = "get";
 constexpr const char *kArgumentAlpha = "alpha";
 constexpr const char *kArgumentEpsilon = "epsilon";
-constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldRank = "rank";
 
 struct ViewGraph {
@@ -85,55 +84,26 @@ ViewGraph PullGraphView(mgp_graph *graph, mgp_memory *memory) {
   return vg;
 }
 
-void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, double centrality) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return;
-  }
-  OwnedValue node;
-  Check(mgp_value_make_vertex(vertex, &node.v));  // takes ownership of `vertex` on success
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
-  Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  OwnedValue value;
-  Check(mgp_value_make_double(centrality, memory, &value.v));
-  Check(mgp_result_record_insert(record, kFieldRank, value.v));
-}
-
 void GetKatzCentrality(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    mgp_value *arg = nullptr;
-    double alpha = 0.0, epsilon = 0.0;
-    Check(mgp_list_at(args, 0, &arg));
-    Check(mgp_value_get_double(arg, &alpha));
-    Check(mgp_list_at(args, 1, &arg));
-    Check(mgp_value_get_double(arg, &epsilon));
+  mgp_value *arg = nullptr;
+  double alpha = 0.0, epsilon = 0.0;
+  Check(mgp_list_at(args, 0, &arg));
+  Check(mgp_value_get_double(arg, &alpha));
+  Check(mgp_list_at(args, 1, &arg));
+  Check(mgp_value_get_double(arg, &epsilon));
 
-    const ViewGraph vg = PullGraphView(graph, memory);
-    const uint64_t n = vg.gid_of_dense.size();
-    std::vector<double> centralities(n, 0.0);
-    uint64_t iterations = 0;
-    // max_iterations = 0: like the reference, the loop ends only when the ranking has separated (katz.cpp:250)
-    if (n != 0) {  // an empty view yields zero rows in the reference too; nothing to compute anywhere
-      const int rc = mgb200_katz_centrality(n, vg.from.size(), vg.from.data(), vg.to.data(), alpha, epsilon, 0,
-                                            centralities.data(), &iterations);
-      if (rc != MGB200_OK) throw ModuleError(mgb200_last_error());
-    }
+  const ViewGraph vg = PullGraphView(graph, memory);
+  const uint64_t n = vg.gid_of_dense.size();
+  std::vector<double> centralities(n, 0.0);
+  uint64_t iterations = 0;
+  // max_iterations = 0: like the reference, the loop ends only when the ranking has separated (katz.cpp:250)
+  if (n != 0)  // an empty view yields zero rows in the reference too; nothing to compute anywhere
+    CheckDevice(mgb200_katz_centrality(n, vg.from.size(), vg.from.data(), vg.to.data(), alpha, epsilon, 0,
+                                       centralities.data(), &iterations));
 
-    if (mgp_result_reserve != nullptr && n != 0) (void)mgp_result_reserve(result, n);
-    for (uint64_t dense = 0; dense < n; ++dense)
-      EmitRecord(graph, result, memory, vg.gid_of_dense[dense], centralities[dense]);
-  } catch (const std::exception &e) {
-    (void)mgp_result_set_error_msg(result, e.what());  // nothing may escape the callback (reference :49-52)
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
-  }
+  if (mgp_result_reserve != nullptr && n != 0) (void)mgp_result_reserve(result, n);
+  for (uint64_t dense = 0; dense < n; ++dense)
+    EmitNodeRow(graph, result, memory, vg.gid_of_dense[dense], kFieldRank, centralities[dense]);
 }
 
 }  // namespace
@@ -144,7 +114,7 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   OwnedValue default_alpha, default_epsilon;  // both destroyed on every path (the reference destroys alpha twice, :72-73)
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, kProcedureGet, GetKatzCentrality, &proc));
+    Check(mgp_module_add_read_procedure(module, kProcedureGet, Guarded<GetKatzCentrality>, &proc));
     Check(mgp_value_make_double(0.2, memory, &default_alpha.v));
     Check(mgp_value_make_double(1e-2, memory, &default_epsilon.v));
     mgp_type *type_float = nullptr, *type_node = nullptr;

@@ -1,6 +1,7 @@
 // memgraph_b200/csrc/mgp_module_common.hpp -- host-side pieces shared by the query modules (pagerank.so, gpu_bfs.so, ...):
-// mgp_error -> exception with the reference's texts, owning iterator wrappers, and the one-pass graph pull through
-// the mgp_graph iterators (the reference's CreatePageRankGraph, mage/cpp/pagerank_module/pagerank_module.cpp:18-54).
+// mgp_error -> exception with the reference's texts, owning iterator wrappers, the one-pass graph pull through
+// the mgp_graph iterators (the reference's CreatePageRankGraph, mage/cpp/pagerank_module/pagerank_module.cpp:18-54),
+// and the per-call glue around the algorithm: device choice, device-graph handles, rows and the error boundary.
 #pragma once
 
 #include <cstdint>
@@ -12,6 +13,8 @@
 #include <type_traits>
 #include <vector>
 
+#include "mgb200_bfs.h"
+#include "mgb200_personalized.h"
 #include "mgp_abi.h"
 
 #ifdef MGB200_USE_REFERENCE_MGP_HEADER
@@ -255,6 +258,119 @@ inline HostGraph PullGraph(mgp_graph *graph, mgp_memory *memory, UnknownGid poli
   hg.to.resize(kept);
   if constexpr (kRead) edge_values->resize(kept);
   return hg;
+}
+
+// ---- per-call glue: the device, the device-graph handles, the rows and the callback's error boundary ----------------
+
+// The device a module's call runs on: MGB200_DEVICE, default 0.
+inline int DeviceFromEnv() {
+  const char *dev_env = std::getenv("MGB200_DEVICE");
+  return dev_env ? std::atoi(dev_env) : 0;
+}
+
+// A device call's nonzero return code as a ModuleError with mgb200_last_error()'s text.  The text is copied into the
+// exception before any handle is destroyed by the unwinding, so a destroy cannot overwrite it.
+inline void CheckDevice(int rc) {
+  if (rc != MGB200_OK) throw ModuleError(mgb200_last_error());
+}
+
+// The `should_abort` poll the device loops take: the host's mgp_must_abort for the graph passed as `user`.
+inline int MustAbortPoll(void *user) { return MustAbort(static_cast<mgp_graph *>(user)) ? 1 : 0; }
+
+// Owns one device-graph handle (null until a create call fills `h`); Release() hands it to an owner that outlives the
+// call, such as the PageRank module's graph cache.
+template <typename T, void (*Destroy)(T *)>
+struct DeviceHandle {
+  T *h = nullptr;
+  DeviceHandle() = default;
+  ~DeviceHandle() { Destroy(h); }
+  T *Release() {
+    T *released = h;
+    h = nullptr;
+    return released;
+  }
+  DeviceHandle(const DeviceHandle &) = delete;
+  DeviceHandle &operator=(const DeviceHandle &) = delete;
+};
+using DeviceGraph = DeviceHandle<mgb200_graph, mgb200_graph_destroy>;
+using BfsGraph = DeviceHandle<mgb200_bfs_graph, mgb200_bfs_graph_destroy>;
+using HitsGraph = DeviceHandle<mgb200_hits_graph, mgb200_hits_graph_destroy>;
+
+// A pulled graph uploaded as a BFS device graph on DeviceFromEnv().  The upload takes 64-bit endpoints, so the edges are
+// widened once into `from` / `to`; biconnectivity and gpu_wsp pass the same arrays on to their later calls.
+struct BfsDeviceGraph {
+  std::vector<uint64_t> from, to;
+  BfsGraph graph;
+  explicit BfsDeviceGraph(const HostGraph &hg) : from(hg.from.begin(), hg.from.end()), to(hg.to.begin(), hg.to.end()) {
+    CheckDevice(mgb200_bfs_graph_create_host(DeviceFromEnv(), hg.gid_of_dense.size(), from.size(), from.data(),
+                                             to.data(), &graph.h));
+  }
+};
+
+constexpr const char *kFieldNode = "node";
+
+// The vertex `gid` as a value in *out; false when it has vanished in analytical mode (the row is skipped), "Invalid ID!"
+// in transactional mode (mg_utility::GetNodeForInsertion).
+inline bool NodeValue(mgp_graph *graph, mgp_memory *memory, int64_t gid, OwnedValue *out) {
+  mgp_vertex *vertex = nullptr;
+  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
+  if (vertex == nullptr) {
+    int transactional = 0;
+    Check(mgp_graph_is_transactional(graph, &transactional));
+    if (transactional) throw ModuleError("Invalid ID!");
+    return false;
+  }
+  Check(mgp_value_make_vertex(vertex, &out->v));  // takes ownership of `vertex` on success
+  return true;
+}
+
+inline mgp_result_record *NewRecord(mgp_result *result) {
+  mgp_result_record *record = nullptr;
+  Check(mgp_result_new_record(result, &record));
+  if (record == nullptr)
+    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
+  return record;
+}
+
+inline void InsertColumns(mgp_result_record *, mgp_memory *) {}
+
+// (name, value) pairs: a floating-point value becomes a FLOAT column, an integer an INTEGER column.  Only the mgp_value_make_*
+// a module's columns need is instantiated, so a module imports nothing it does not use.
+template <typename T, typename... Rest>
+void InsertColumns(mgp_result_record *record, mgp_memory *memory, const char *field, T value, Rest... rest) {
+  OwnedValue column;
+  if constexpr (std::is_floating_point_v<T>) {
+    Check(mgp_value_make_double(value, memory, &column.v));
+  } else {
+    static_assert(std::is_integral_v<T>);
+    Check(mgp_value_make_int(value, memory, &column.v));
+  }
+  Check(mgp_result_record_insert(record, field, column.v));
+  InsertColumns(record, memory, rest...);
+}
+
+// One row: `node` (the vertex `gid`), then the (name, value) columns in order.  No row when the vertex has vanished in
+// analytical mode (NodeValue).
+template <typename... Columns>
+void EmitNodeRow(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, Columns... columns) {
+  OwnedValue node;
+  if (!NodeValue(graph, memory, gid, &node)) return;
+  mgp_result_record *record = NewRecord(result);
+  Check(mgp_result_record_insert(record, kFieldNode, node.v));
+  InsertColumns(record, memory, columns...);
+}
+
+// The procedure callback around `Body`: nothing may escape it, so an exception becomes the procedure's error message,
+// which the engine reports as QueryRuntimeException("<module>.<procedure>: <message>").
+template <void (*Body)(mgp_list *, mgp_graph *, mgp_result *, mgp_memory *)>
+void Guarded(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
+  try {
+    Body(args, graph, result, memory);
+  } catch (const std::exception &e) {
+    (void)mgp_result_set_error_msg(result, e.what());
+  } catch (...) {
+    (void)mgp_result_set_error_msg(result, "Unknown exception!");
+  }
 }
 
 

@@ -29,7 +29,6 @@ using namespace mgb200_module;
 namespace {
 
 constexpr const char *kProcedureGet = "get";
-constexpr const char *kFieldNode = "node";
 constexpr const char *kFieldRank = "rank";
 constexpr const char *kArgMaxIterations = "max_iterations";
 constexpr const char *kArgDampingFactor = "damping_factor";
@@ -44,8 +43,6 @@ struct DeviceGraphCache {
   ~DeviceGraphCache() { mgb200_graph_destroy(graph); }
 };
 
-int AbortTrampoline(void *user) { return MustAbort(static_cast<mgp_graph *>(user)) ? 1 : 0; }
-
 std::vector<double> ComputeRanks(const HostGraph &hg, mgp_graph *graph, int64_t max_iterations, double damping_factor,
                                  double stop_epsilon, int64_t num_threads) {
   // pagerank.hpp:109 takes uint32_t, pagerank.cpp:195 clamps to hardware_concurrency, :63-65 rejects 0.
@@ -58,20 +55,18 @@ std::vector<double> ComputeRanks(const HostGraph &hg, mgp_graph *graph, int64_t 
   params.max_iterations = static_cast<uint64_t>(max_iterations);  // int64 -> size_t wrap, reference :95
   params.damping_factor = damping_factor;
   params.stop_epsilon = stop_epsilon;
-  params.should_abort = AbortTrampoline;  // polled between iteration batches, from this thread only
+  params.should_abort = MustAbortPoll;  // polled between iteration batches, from this thread only
   params.abort_user = graph;
   // MGB200_GPUS=P (2..8): vertex-partition the call over GPUs 0..P-1 (device-side exchange over NVLink)
   const char *gpus_env = std::getenv("MGB200_GPUS");
   const int gpus = gpus_env ? std::atoi(gpus_env) : 1;
   if (gpus > 1) {
     uint64_t iterations = 0;
-    const int rc = mgb200_pagerank_multi_u32(n, hg.from.size(), hg.from.data(), hg.to.data(), &params, threads,
-                                             static_cast<uint32_t>(gpus), nullptr, ranks.data(), &iterations);
-    if (rc != MGB200_OK) throw ModuleError(mgb200_last_error());
+    CheckDevice(mgb200_pagerank_multi_u32(n, hg.from.size(), hg.from.data(), hg.to.data(), &params, threads,
+                                          static_cast<uint32_t>(gpus), nullptr, ranks.data(), &iterations));
     return ranks;
   }
-  const char *dev_env = std::getenv("MGB200_DEVICE");
-  const int device = dev_env ? std::atoi(dev_env) : 0;
+  const int device = DeviceFromEnv();
   // MGB200_GRAPH_CACHE=1: keep the device-resident graph across CALLs.  The mgp ABI has no graph version, so the key is a
   // 128-bit fingerprint of the dense COO just pulled (plus n, m, device): an unchanged graph skips the upload and the
   // device build, a changed one replaces the slot.  One slot, taken with try_lock: a concurrent second query (the module is
@@ -80,94 +75,58 @@ std::vector<double> ComputeRanks(const HostGraph &hg, mgp_graph *graph, int64_t 
   const char *cache_env = std::getenv("MGB200_GRAPH_CACHE");
   std::unique_lock<std::mutex> slot(cache.busy, std::defer_lock);
   const bool use_cache = cache_env && cache_env[0] == '1' && slot.try_lock();
+  DeviceGraph owned;  // the handle of a call that does not hand it to the cache
   mgb200_graph *dg = nullptr;
-  bool owned = true;
   if (use_cache) {
     uint64_t fp[2] = {0, 0};
-    if (mgb200_coo_fingerprint_u32(n, hg.from.size(), hg.from.data(), hg.to.data(), fp) != MGB200_OK)
-      throw ModuleError(mgb200_last_error());
+    CheckDevice(mgb200_coo_fingerprint_u32(n, hg.from.size(), hg.from.data(), hg.to.data(), fp));
     if (cache.graph && cache.n == n && cache.m == hg.from.size() && cache.device == device && cache.fp[0] == fp[0] &&
         cache.fp[1] == fp[1]) {
-      dg = cache.graph;
       ++cache.hits;
     } else {
       mgb200_graph_destroy(cache.graph);
       cache.graph = nullptr;
-      if (mgb200_graph_create_host_u32(device, n, hg.from.size(), hg.from.data(), hg.to.data(), 0, 1, &dg) != MGB200_OK)
-        throw ModuleError(mgb200_last_error());
-      cache.graph = dg;
+      CheckDevice(mgb200_graph_create_host_u32(device, n, hg.from.size(), hg.from.data(), hg.to.data(), 0, 1, &owned.h));
+      cache.graph = owned.Release();
       cache.n = n;
       cache.m = hg.from.size();
       cache.device = device;
       cache.fp[0] = fp[0];
       cache.fp[1] = fp[1];
     }
-    owned = false;
-  } else if (mgb200_graph_create_host_u32(device, n, hg.from.size(), hg.from.data(), hg.to.data(), 0, 1, &dg) != MGB200_OK) {
-    throw ModuleError(mgb200_last_error());
+    dg = cache.graph;
+  } else {
+    CheckDevice(mgb200_graph_create_host_u32(device, n, hg.from.size(), hg.from.data(), hg.to.data(), 0, 1, &owned.h));
+    dg = owned.h;
   }
   mgb200_run_stats stats{};
-  const int rc = mgb200_pagerank_run(dg, &params, ranks.data(), &stats);
-  const std::string message = rc != MGB200_OK ? mgb200_last_error() : "";
-  if (owned) mgb200_graph_destroy(dg);
-  if (rc != MGB200_OK) throw ModuleError(message);
+  CheckDevice(mgb200_pagerank_run(dg, &params, ranks.data(), &stats));
   return ranks;
 }
 
-// One (node, rank) row (reference InsertPagerankRecord :69-84).  Returns false when the vertex has
-// vanished in analytical mode (row skipped), throws "Invalid ID!" in transactional mode.
-void EmitRecord(mgp_graph *graph, mgp_result *result, mgp_memory *memory, int64_t gid, double rank) {
-  mgp_vertex *vertex = nullptr;
-  Check(mgp_graph_get_vertex_by_id(graph, mgp_vertex_id{gid}, memory, &vertex));
-  if (vertex == nullptr) {
-    int transactional = 0;
-    Check(mgp_graph_is_transactional(graph, &transactional));
-    if (transactional) throw ModuleError("Invalid ID!");
-    return;
-  }
-  OwnedValue node;
-  {
-    const mgp_error e = mgp_value_make_vertex(vertex, &node.v);  // takes ownership of `vertex` on success
-    if (e != mgp_error::MGP_ERROR_NO_ERROR) Check(e);
-  }
-  mgp_result_record *record = nullptr;
-  Check(mgp_result_new_record(result, &record));
-  if (record == nullptr)
-    throw ModuleError("Not enough memory! For more details please visit https://memgr.ph/memory-control");
-  Check(mgp_result_record_insert(record, kFieldNode, node.v));
-  OwnedValue value;
-  Check(mgp_value_make_double(rank, memory, &value.v));
-  Check(mgp_result_record_insert(record, kFieldRank, value.v));
-}
-
+// Nothing may escape the callback (reference :108-112); Guarded turns an exception into the error message, which the
+// engine reports as QueryRuntimeException("pagerank.get: <msg>") (src/query/plan/operator.cpp:7929-7932).
 void PagerankGet(mgp_list *args, mgp_graph *graph, mgp_result *result, mgp_memory *memory) {
-  try {
-    mgp_value *arg = nullptr;
-    int64_t max_iterations = 0, num_threads = 0;
-    double damping_factor = 0.0, stop_epsilon = 0.0;
-    Check(mgp_list_at(args, 0, &arg));
-    Check(mgp_value_get_int(arg, &max_iterations));
-    Check(mgp_list_at(args, 1, &arg));
-    Check(mgp_value_get_double(arg, &damping_factor));
-    Check(mgp_list_at(args, 2, &arg));
-    Check(mgp_value_get_double(arg, &stop_epsilon));
-    Check(mgp_list_at(args, 3, &arg));
-    Check(mgp_value_get_int(arg, &num_threads));
+  mgp_value *arg = nullptr;
+  int64_t max_iterations = 0, num_threads = 0;
+  double damping_factor = 0.0, stop_epsilon = 0.0;
+  Check(mgp_list_at(args, 0, &arg));
+  Check(mgp_value_get_int(arg, &max_iterations));
+  Check(mgp_list_at(args, 1, &arg));
+  Check(mgp_value_get_double(arg, &damping_factor));
+  Check(mgp_list_at(args, 2, &arg));
+  Check(mgp_value_get_double(arg, &stop_epsilon));
+  Check(mgp_list_at(args, 3, &arg));
+  Check(mgp_value_get_int(arg, &num_threads));
 
-    const HostGraph hg = PullGraph(graph, memory);
-    const std::vector<double> ranks =
-        ComputeRanks(hg, graph, max_iterations, damping_factor, stop_epsilon, num_threads);
+  const HostGraph hg = PullGraph(graph, memory);
+  const std::vector<double> ranks =
+      ComputeRanks(hg, graph, max_iterations, damping_factor, stop_epsilon, num_threads);
 
-    if (mgp_result_reserve != nullptr && !ranks.empty()) (void)mgp_result_reserve(result, ranks.size());
-    for (std::size_t dense = 0; dense < ranks.size(); ++dense)
-      EmitRecord(graph, result, memory, hg.gid_of_dense[dense], ranks[dense]);
-  } catch (const std::exception &e) {
-    // Nothing may escape the callback (reference :108-112); the engine turns the message into
-    // QueryRuntimeException("pagerank.get: <msg>") (src/query/plan/operator.cpp:7929-7932).
-    (void)mgp_result_set_error_msg(result, e.what());
-  } catch (...) {
-    (void)mgp_result_set_error_msg(result, "Unknown exception!");
-  }
+  if (mgp_result_reserve != nullptr && !ranks.empty()) (void)mgp_result_reserve(result, ranks.size());
+  // one (node, rank) row per vertex (reference InsertPagerankRecord :69-84)
+  for (std::size_t dense = 0; dense < ranks.size(); ++dense)
+    EmitNodeRow(graph, result, memory, hg.gid_of_dense[dense], kFieldRank, ranks[dense]);
 }
 
 }  // namespace
@@ -178,7 +137,7 @@ __attribute__((visibility("default"))) int mgp_init_module(struct mgp_module *mo
   OwnedValue max_iterations, damping_factor, stop_epsilon, num_threads;  // destroyed on every path (:139-152)
   try {
     mgp_proc *proc = nullptr;
-    Check(mgp_module_add_read_procedure(module, kProcedureGet, PagerankGet, &proc));
+    Check(mgp_module_add_read_procedure(module, kProcedureGet, Guarded<PagerankGet>, &proc));
     Check(mgp_value_make_int(100, memory, &max_iterations.v));
     Check(mgp_value_make_double(0.85, memory, &damping_factor.v));
     Check(mgp_value_make_double(1e-5, memory, &stop_epsilon.v));
