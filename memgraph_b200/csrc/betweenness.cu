@@ -36,9 +36,7 @@ namespace mgb200 {
 namespace {
 
 constexpr int S = MGB200_BC_BATCH;
-constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr unsigned kFull = 0xffffffffu;
 constexpr uint64_t kHeavyDegree = 512;  // above this, one block (8 warps) per vertex instead of one warp
 constexpr int kLoadsInFlight = 8;        // candidate edges whose rows a warp loads before it adds any of them
 constexpr int kLevelsPerSync = 8;
@@ -336,26 +334,6 @@ __global__ void heavy_list_kernel(uint64_t n, Lists lists, uint32_t *out, unsign
     if (lists.degree(static_cast<uint32_t>(v)) > kHeavyDegree) out[atomicAdd(count, 1u)] = static_cast<uint32_t>(v);
 }
 
-int grid_for(uint64_t threads_wanted, int sm_count, int per_sm = 16) {
-  const uint64_t want = (threads_wanted + kThreads - 1) / kThreads;
-  return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * per_sm)));
-}
-
-struct Buffers {
-  std::vector<void *> ptrs;
-  ~Buffers() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 }  // namespace
 }  // namespace mgb200
 
@@ -382,7 +360,7 @@ int mgb200_bc_run(mgb200_bfs_graph *g, int directed, uint64_t source_begin, uint
   stats.sources = source_end - source_begin;
   stats.batch_width = S;
 
-  Buffers buf;
+  DeviceBuffers buf;
   State st{};
   double *bc = nullptr;
   uint32_t *heavy_pull = nullptr, *heavy_push = nullptr;
@@ -414,8 +392,8 @@ int mgb200_bc_run(mgb200_bfs_graph *g, int directed, uint64_t source_begin, uint
   MGB_CUDA(cudaMemsetAsync(st.inspected, 0, sizeof(unsigned long long), st_));
   MGB_CUDA(cudaMemsetAsync(heavy_count, 0, 2 * sizeof(unsigned int), st_));
   if (n) {
-    heavy_list_kernel<<<grid_for(n, g->sm_count), kThreads, 0, st_>>>(n, pull, heavy_pull, heavy_count);
-    heavy_list_kernel<<<grid_for(n, g->sm_count), kThreads, 0, st_>>>(n, push, heavy_push, heavy_count + 1);
+    heavy_list_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st_>>>(n, pull, heavy_pull, heavy_count);
+    heavy_list_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st_>>>(n, push, heavy_push, heavy_count + 1);
     stats.kernel_launches += 2;
   }
   unsigned int n_heavy[2] = {0, 0};
@@ -423,7 +401,7 @@ int mgb200_bc_run(mgb200_bfs_graph *g, int directed, uint64_t source_begin, uint
   MGB_CUDA(cudaStreamSynchronize(st_));
   MGB_CUDA(cudaGetLastError());
 
-  const int warp_grid = grid_for(n * 32, g->sm_count, 8);
+  const int warp_grid = blocks_for(n * 32, g->sm_count, 8);
   std::vector<unsigned long long> off_host;
   std::vector<uint32_t> cnt_host;
   for (uint64_t s0 = source_begin; s0 < source_end; s0 += S) {
@@ -433,7 +411,7 @@ int mgb200_bc_run(mgb200_bfs_graph *g, int directed, uint64_t source_begin, uint
     }
     const uint32_t width = static_cast<uint32_t>(std::min<uint64_t>(S, source_end - s0));
     const uint32_t lane_mask = width == 32 ? kFull : (1u << width) - 1u;
-    init_batch_kernel<<<grid_for(n, g->sm_count), kThreads, 0, st_>>>(n, s0, width, st);
+    init_batch_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st_>>>(n, s0, width, st);
     stats.kernel_launches++;
     // forward: groups of levels, then one read of their frontier sizes
     int deepest = 0;
@@ -473,7 +451,7 @@ int mgb200_bc_run(mgb200_bfs_graph *g, int directed, uint64_t source_begin, uint
     // backward: deepest level first; the sources' own level 0 has no dependency to add
     for (int level = deepest; level >= 1; --level) {
       if (cnt_host[level]) {
-        backward_kernel<<<grid_for(static_cast<uint64_t>(cnt_host[level]) * 32, g->sm_count, 8), kThreads, 0, st_>>>(
+        backward_kernel<<<blocks_for(static_cast<uint64_t>(cnt_host[level]) * 32, g->sm_count, 8), kThreads, 0, st_>>>(
             st.list + off_host[level], cnt_host[level], push, level, st);
         stats.kernel_launches++;
       }

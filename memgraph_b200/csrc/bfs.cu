@@ -23,14 +23,7 @@
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr uint32_t kSegEdges = 1024;
-constexpr unsigned kFull = 0xffffffffu;
-
-inline int blocks_for(uint64_t items, int sm_count, int per_sm = 16) {
-  const uint64_t want = (items + kThreads - 1) / kThreads;
-  return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * per_sm)));
-}
 
 struct Adj {  // the adjacency a direction walks: `a` first, then `b` (BOTH)
   const uint64_t *a_ptr;
@@ -198,23 +191,8 @@ __global__ void finalize_kernel(uint64_t n, uint32_t source, const int32_t *dept
   }
 }
 
-struct Scratch {
-  std::vector<void *> ptrs;
-  ~Scratch() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 // rows sorted by (row, neighbour): ptr from the degree counts, adj from the sorted keys
-int build_side(mgb200_bfs_graph &g, Scratch &tmp, const uint32_t *row, const uint32_t *col,
+int build_side(mgb200_bfs_graph &g, DeviceBuffers &tmp, const uint32_t *row, const uint32_t *col,
                const unsigned long long *deg, uint64_t **ptr_out, uint32_t **adj_out) {
   const uint64_t n = g.n, m = g.m;
   cudaStream_t st = g.stream;
@@ -232,7 +210,7 @@ int build_side(mgb200_bfs_graph &g, Scratch &tmp, const uint32_t *row, const uin
   uint64_t *key = nullptr, *alt = nullptr;
   MGB_CUDA(tmp.alloc(&key, m));
   MGB_CUDA(tmp.alloc(&alt, m));
-  pair_key_kernel<<<blocks_for(m, g.sm_count), kThreads, 0, st>>>(m, row, col, key);
+  pair_key_kernel<<<blocks_for(m, g.sm_count, 16), kThreads, 0, st>>>(m, row, col, key);
   cub::DoubleBuffer<uint64_t> kb(key, alt);
   size_t bytes = 0;
   int bits = 1;
@@ -241,7 +219,7 @@ int build_side(mgb200_bfs_graph &g, Scratch &tmp, const uint32_t *row, const uin
   void *t = nullptr;
   MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&t), bytes));
   MGB_CUDA(cub::DeviceRadixSort::SortKeys(t, bytes, kb, m, 0, 32 + bits, st));
-  low_half_kernel<<<blocks_for(m, g.sm_count), kThreads, 0, st>>>(m, kb.Current(), *adj_out);
+  low_half_kernel<<<blocks_for(m, g.sm_count, 16), kThreads, 0, st>>>(m, kb.Current(), *adj_out);
   MGB_CUDA(cudaGetLastError());
   MGB_CUDA(cudaStreamSynchronize(st));
   return MGB200_OK;
@@ -307,7 +285,7 @@ int mgb200_bfs_graph_create_device(int device, uint64_t n, uint64_t m, const uin
     MGB_CUDA(cudaEventCreate(&g->ev0));
     MGB_CUDA(cudaEventCreate(&g->ev1));
     cudaStream_t st = g->stream;
-    Scratch tmp;
+    DeviceBuffers tmp;
     unsigned long long *out_deg = nullptr, *in_deg = nullptr;
     int *bad = nullptr;
     MGB_CUDA(tmp.alloc(&out_deg, n + 1));
@@ -316,7 +294,7 @@ int mgb200_bfs_graph_create_device(int device, uint64_t n, uint64_t m, const uin
     MGB_CUDA(cudaMemsetAsync(out_deg, 0, (n + 1) * sizeof(unsigned long long), st));
     MGB_CUDA(cudaMemsetAsync(in_deg, 0, (n + 1) * sizeof(unsigned long long), st));
     MGB_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
-    if (m) degree_count_kernel<<<blocks_for(m, g->sm_count), kThreads, 0, st>>>(m, n, d_from, d_to, out_deg, in_deg, bad);
+    if (m) degree_count_kernel<<<blocks_for(m, g->sm_count, 16), kThreads, 0, st>>>(m, n, d_from, d_to, out_deg, in_deg, bad);
     int bad_host = 0;
     MGB_CUDA(cudaMemcpyAsync(&bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
@@ -373,23 +351,15 @@ int mgb200_bfs_graph_create_host(int device, uint64_t n, uint64_t m, const uint6
     return MGB200_ERR_CUDA;
   }
   MGB_CUDA(cudaSetDevice(device));
+  DeviceBuffers coo;
   uint32_t *d_f = nullptr, *d_t = nullptr;
-  MGB_CUDA(cudaMalloc(&d_f, std::max<uint64_t>(m, 1) * 4));
-  cudaError_t e2 = cudaMalloc(&d_t, std::max<uint64_t>(m, 1) * 4);
-  if (e2 != cudaSuccess) {
-    cudaFree(d_f);
-    return cuda_fail(e2, "cudaMalloc", __FILE__, __LINE__);
-  }
-  int rc = MGB200_OK;
+  MGB_CUDA(coo.alloc(&d_f, m));
+  MGB_CUDA(coo.alloc(&d_t, m));
   if (m) {
-    cudaError_t a = cudaMemcpy(d_f, f.data(), m * 4, cudaMemcpyHostToDevice);
-    cudaError_t b = cudaMemcpy(d_t, t.data(), m * 4, cudaMemcpyHostToDevice);
-    if (a != cudaSuccess || b != cudaSuccess) rc = cuda_fail(a != cudaSuccess ? a : b, "cudaMemcpy(COO)", __FILE__, __LINE__);
+    MGB_CUDA(cudaMemcpy(d_f, f.data(), m * 4, cudaMemcpyHostToDevice));
+    MGB_CUDA(cudaMemcpy(d_t, t.data(), m * 4, cudaMemcpyHostToDevice));
   }
-  if (!rc) rc = mgb200_bfs_graph_create_device(device, n, m, d_f, d_t, out);
-  cudaFree(d_f);
-  cudaFree(d_t);
-  return rc;
+  return mgb200_bfs_graph_create_device(device, n, m, d_f, d_t, out);
 }
 
 int mgb200_bfs_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t lower_bound, int64_t upper_bound,
@@ -421,7 +391,7 @@ int mgb200_bfs_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
   const uint64_t words = (n + 31) / 32;
 
   MGB_CUDA(cudaEventRecord(g->ev0, st));
-  init_depth_kernel<<<blocks_for(n, g->sm_count), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), g->depth,
+  init_depth_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), g->depth,
                                                                      g->queue[0], g->counters);
   stats.kernel_launches++;
   uint64_t nf = 1;
@@ -431,7 +401,7 @@ int mgb200_bfs_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
   const bool bounds_empty = upper_bound < 1 || lower_bound > upper_bound;  // operator.cpp:2830
   while (!bounds_empty && nf > 0 && static_cast<int64_t>(level) < upper_bound && level < INT_MAX - 1) {
     // frontier statistics: segments per vertex and degree sum (m_f)
-    frontier_segments_kernel<<<blocks_for(nf, g->sm_count), kThreads, 0, st>>>(nf, g->queue[cur], forward, g->seg_count,
+    frontier_segments_kernel<<<blocks_for(nf, g->sm_count, 16), kThreads, 0, st>>>(nf, g->queue[cur], forward, g->seg_count,
                                                                                 g->counters);
     int rc = read_counters(*g);
     if (rc) return rc;
@@ -443,8 +413,8 @@ int mgb200_bfs_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
     const bool bottom_up = m_f > m_u / 14 && nf > 1024;
     MGB_CUDA(cudaMemsetAsync(g->counters, 0, 2 * sizeof(unsigned long long), st));
     if (bottom_up) {
-      clear_words_kernel<<<blocks_for(words, g->sm_count), kThreads, 0, st>>>(words, g->bitmap[0]);
-      queue_to_bitmap_kernel<<<blocks_for(nf, g->sm_count), kThreads, 0, st>>>(nf, g->queue[cur], g->bitmap[0]);
+      clear_words_kernel<<<blocks_for(words, g->sm_count, 16), kThreads, 0, st>>>(words, g->bitmap[0]);
+      queue_to_bitmap_kernel<<<blocks_for(nf, g->sm_count, 16), kThreads, 0, st>>>(nf, g->queue[cur], g->bitmap[0]);
       bottom_up_kernel<<<blocks_for(n, g->sm_count, 32), kThreads, 0, st>>>(n, reverse, g->bitmap[0], level + 1, g->depth,
                                                                             g->queue[cur ^ 1], g->counters);
       stats.kernel_launches += 3;
@@ -470,7 +440,7 @@ int mgb200_bfs_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
   if (n > 0) {
     int32_t *d_out = dist_out;
     if (!dist_on_device) MGB_CUDA(cudaMalloc(&d_out, n * sizeof(int32_t)));
-    finalize_kernel<<<blocks_for(n, g->sm_count), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), g->depth,
+    finalize_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), g->depth,
                                                                     static_cast<long long>(lower_bound),
                                                                     static_cast<long long>(upper_bound), d_out);
     stats.kernel_launches++;

@@ -1,6 +1,7 @@
 // memgraph_b200/csrc/bfs_graph.hpp -- the device graph behind the opaque mgb200_bfs_graph handle (include/mgb200_bfs.h).
 // Shared by the breadth-first expansion (bfs.cu), which builds it, betweenness centrality (betweenness.cu), weakly
-// connected components (wcc.cu) and weighted shortest paths (wsp.cu), which walk the same CSR + CSC.
+// connected components (wcc.cu), bridges and biconnected components (biconnectivity.cu) and weighted shortest paths
+// (wsp.cu), which walk the same CSR + CSC; also the grid-stride and warp helpers of their kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -30,3 +31,23 @@ struct mgb200_bfs_graph {
   size_t cub_tmp_bytes = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 };
+
+namespace mgb200 {
+namespace {
+
+constexpr unsigned kFull = 0xffffffffu;
+
+__device__ __forceinline__ uint64_t first_thread() { return static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; }
+__device__ __forceinline__ uint64_t thread_count() { return static_cast<uint64_t>(gridDim.x) * blockDim.x; }
+
+// Grid-stride loops that shuffle run whole warps (the bound is rounded up to a multiple of 32) so the shuffles see
+// every lane.
+__device__ __forceinline__ uint64_t warp_rounded(uint64_t n) { return (n + 31) & ~31ull; }
+
+__device__ __forceinline__ void add_warp_sum(unsigned long long x, unsigned long long *counter) {
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(kFull, x, o);
+  if ((threadIdx.x & 31) == 0 && x) atomicAdd(counter, x);
+}
+
+}  // namespace
+}  // namespace mgb200

@@ -42,8 +42,6 @@ namespace cg = cooperative_groups;
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr unsigned kFull = 0xffffffffu;
 constexpr uint32_t kNone = 0xffffffffu;
 constexpr uint64_t kThreadEntries = 16;  // entries a single thread walks
 constexpr uint64_t kWarpEntries = 4096;  // above this, a block per vertex
@@ -71,15 +69,6 @@ struct Counters {
   unsigned long long components;
   unsigned long long trees;
 };
-
-__device__ __forceinline__ uint64_t first_thread() { return static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; }
-__device__ __forceinline__ uint64_t thread_count() { return static_cast<uint64_t>(gridDim.x) * blockDim.x; }
-__device__ __forceinline__ uint64_t warp_rounded(uint64_t n) { return (n + 31) & ~31ull; }
-
-__device__ __forceinline__ void add_warp_sum(unsigned long long x, unsigned long long *counter) {
-  for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(kFull, x, o);
-  if ((threadIdx.x & 31) == 0 && x) atomicAdd(counter, x);
-}
 
 // Appends w to dst at a slot reserved with one atomic per group of converged threads.
 __device__ __forceinline__ void append(uint32_t w, uint32_t *dst, unsigned long long *counter) {
@@ -381,35 +370,15 @@ __global__ void __launch_bounds__(kThreads) number_kernel(uint64_t m, const uint
   add_warp_sum(firsts, &counters->components);
 }
 
-int grid_for(uint64_t threads_wanted, int sm_count, int per_sm = 8) {
-  const uint64_t want = (threads_wanted + kThreads - 1) / kThreads;
-  return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * per_sm)));
-}
-
-struct Buffers {
-  std::vector<void *> ptrs;
-  ~Buffers() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 // One entry-scan pass over items [lo, hi): thread, warp and block kernels.
 template <class Op>
 void walk(const mgb200_bfs_graph &g, uint64_t lo, uint64_t hi, const uint32_t *items, const Op &op, uint32_t *work,
           Split *split, Split *clear, Counters *counters, uint64_t *launches) {
   const uint64_t count = hi - lo;
-  walk_thread_kernel<Op><<<grid_for(count, g.sm_count), kThreads, 0, g.stream>>>(lo, hi, items, g.n, op, work, split,
-                                                                                  clear, &counters->inspected);
-  walk_warp_kernel<Op><<<grid_for(count * 32, g.sm_count, 16), kThreads, 0, g.stream>>>(op, work, split,
-                                                                                         &counters->inspected);
+  walk_thread_kernel<Op><<<blocks_for(count, g.sm_count, 8), kThreads, 0, g.stream>>>(
+      lo, hi, items, g.n, op, work, split, clear, &counters->inspected);
+  walk_warp_kernel<Op><<<blocks_for(count * 32, g.sm_count, 16), kThreads, 0, g.stream>>>(op, work, split,
+                                                                                           &counters->inspected);
   walk_block_kernel<Op><<<static_cast<int>(std::min<uint64_t>(count, static_cast<uint64_t>(g.sm_count) * 8)), kThreads,
                           0, g.stream>>>(g.n, op, work, split, &counters->inspected);
   *launches += 3;
@@ -449,7 +418,7 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
   int32_t *depth = g->depth;
   uint32_t *order = g->queue[0], *work = g->queue[1];
 
-  Buffers buf;
+  DeviceBuffers buf;
   uint32_t *d_from = nullptr, *d_to = nullptr, *uf = nullptr, *tree_parent = nullptr, *size = nullptr, *pre = nullptr,
            *low = nullptr, *high = nullptr, *keys = nullptr, *sorted = nullptr, *scan = nullptr, *block = nullptr;
   unsigned long long *first_edge = nullptr;
@@ -497,7 +466,7 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
     MGB_CUDA(cudaMemcpyAsync(d_to, t.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
   }
 
-  const int grid_n = grid_for(n, g->sm_count), grid_m = grid_for(m, g->sm_count);
+  const int grid_n = blocks_for(n, g->sm_count, 8), grid_m = blocks_for(m, g->sm_count, 8);
   uint64_t launches = 0;
   unsigned long long *host_next = g->host_counters;  // pinned
   MGB_CUDA(cudaEventRecord(g->ev0, st));
@@ -536,8 +505,8 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
 
   // subtree sizes, bottom-up
   for (uint32_t L = levels - 1; L >= 1; --L) {
-    size_level_kernel<<<grid_for(level[L + 1] - level[L], g->sm_count), kThreads, 0, st>>>(level[L], level[L + 1],
-                                                                                             order, tree_parent, size);
+    size_level_kernel<<<blocks_for(level[L + 1] - level[L], g->sm_count, 8), kThreads, 0, st>>>(
+        level[L], level[L + 1], order, tree_parent, size);
     ++launches;
   }
   // preorder: roots in root order, siblings in id order, levels top-down
@@ -552,8 +521,8 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
   sibling_kernel<<<grid_n, kThreads, 0, st>>>(n, keys, sorted, run_start, scan, pre);
   launches += 4;
   for (uint32_t L = 1; L < levels; ++L) {
-    pre_level_kernel<<<grid_for(level[L + 1] - level[L], g->sm_count), kThreads, 0, st>>>(level[L], level[L + 1], order,
-                                                                                            tree_parent, pre);
+    pre_level_kernel<<<blocks_for(level[L + 1] - level[L], g->sm_count, 8), kThreads, 0, st>>>(
+        level[L], level[L + 1], order, tree_parent, pre);
     ++launches;
   }
   // low / high: local values, then levels bottom-up
@@ -563,7 +532,7 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
   walk(*g, 0, n, nullptr, LocalOp{lists, pre, tree_parent, low, high}, work, &counters->split[0], nullptr, counters,
        &launches);
   for (uint32_t L = levels - 1; L >= 1; --L) {
-    low_high_level_kernel<<<grid_for(level[L + 1] - level[L], g->sm_count), kThreads, 0, st>>>(
+    low_high_level_kernel<<<blocks_for(level[L + 1] - level[L], g->sm_count, 8), kThreads, 0, st>>>(
         level[L], level[L + 1], order, tree_parent, low, high);
     ++launches;
   }

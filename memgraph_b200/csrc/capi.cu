@@ -151,6 +151,29 @@ int validate_sizes(uint64_t n, uint32_t part_rank, uint32_t part_world) {
   return MGB200_OK;
 }
 
+// A handle for partition part_rank of part_world, built from `edges`; on failure nothing of it is left.
+int new_graph(int device, uint64_t n, uint64_t m, uint32_t part_rank, uint32_t part_world, EdgeSource &edges,
+              mgb200_graph **out) {
+  auto *h = new (std::nothrow) mgb200_graph();
+  if (!h) {
+    set_error("out of host memory");
+    return MGB200_ERR_INVALID_ARGUMENT;
+  }
+  h->g.device = device;
+  h->g.n = n;
+  h->g.m = m;
+  h->g.part_rank = part_rank;
+  h->g.part_world = part_world;
+  const int rc = build_graph(h->g, edges);
+  if (rc) {
+    free_graph(h->g);
+    delete h;
+    return rc;
+  }
+  *out = h;
+  return MGB200_OK;
+}
+
 // Iteration loop shared by the single- and multi-partition entry points.
 int iterate(Graph &g, const mgb200_run_params &p, mgb200_run_stats &stats) {
   MGB_CUDA(cudaSetDevice(g.device));
@@ -304,25 +327,8 @@ int mgb200_graph_create_device(int device, uint64_t n, uint64_t m, const uint32_
   if (rc) return rc;
   rc = check_device(device);
   if (rc) return rc;
-  auto *h = new (std::nothrow) mgb200_graph();
-  if (!h) {
-    set_error("out of host memory");
-    return MGB200_ERR_INVALID_ARGUMENT;
-  }
-  h->g.device = device;
-  h->g.n = n;
-  h->g.m = m;
-  h->g.part_rank = part_rank;
-  h->g.part_world = part_world;
   DeviceArrays source(m, d_from, d_to);
-  rc = build_graph(h->g, source);
-  if (rc) {
-    free_graph(h->g);
-    delete h;
-    return rc;
-  }
-  *out = h;
-  return MGB200_OK;
+  return new_graph(device, n, m, part_rank, part_world, source, out);
 }
 
 int mgb200_graph_create_host_weighted_u32(int device, uint64_t n, uint64_t m, const uint32_t *from, const uint32_t *to,
@@ -348,46 +354,17 @@ int mgb200_graph_create_host_weighted_u32(int device, uint64_t n, uint64_t m, co
       return MGB200_ERR_INVALID_ARGUMENT;
     }
   }
+  DeviceBuffers coo;
   uint32_t *d_from = nullptr, *d_to = nullptr;
   double *d_w = nullptr;
-  auto cleanup = [&]() {
-    cudaFree(d_from);
-    cudaFree(d_to);
-    cudaFree(d_w);
-  };
-  cudaError_t e;
-  const uint64_t cnt = std::max<uint64_t>(m, 1);
-  if ((e = cudaMalloc(&d_from, cnt * 4)) != cudaSuccess || (e = cudaMalloc(&d_to, cnt * 4)) != cudaSuccess ||
-      (e = cudaMalloc(&d_w, cnt * 8)) != cudaSuccess ||
-      (e = cudaMemcpy(d_from, from, m * 4, cudaMemcpyHostToDevice)) != cudaSuccess ||
-      (e = cudaMemcpy(d_to, to, m * 4, cudaMemcpyHostToDevice)) != cudaSuccess ||
-      (e = cudaMemcpy(d_w, weight, m * 8, cudaMemcpyHostToDevice)) != cudaSuccess) {
-    cleanup();
-    return cuda_fail(e, "weighted COO upload", __FILE__, __LINE__);
-  }
-  auto *h = new (std::nothrow) mgb200_graph();
-  if (!h) {
-    cleanup();
-    set_error("out of host memory");
-    return MGB200_ERR_INVALID_ARGUMENT;
-  }
-  h->g.device = device;
-  h->g.n = n;
-  h->g.m = m;
-  h->g.part_rank = 0;
-  h->g.part_world = 1;
-  {
-    DeviceArrays source(m, d_from, d_to, d_w);
-    rc = build_graph(h->g, source);
-  }
-  cleanup();
-  if (rc) {
-    free_graph(h->g);
-    delete h;
-    return rc;
-  }
-  *out = h;
-  return MGB200_OK;
+  MGB_CUDA(coo.alloc(&d_from, m));
+  MGB_CUDA(coo.alloc(&d_to, m));
+  MGB_CUDA(coo.alloc(&d_w, m));
+  MGB_CUDA(cudaMemcpy(d_from, from, m * 4, cudaMemcpyHostToDevice));
+  MGB_CUDA(cudaMemcpy(d_to, to, m * 4, cudaMemcpyHostToDevice));
+  MGB_CUDA(cudaMemcpy(d_w, weight, m * 8, cudaMemcpyHostToDevice));
+  DeviceArrays source(m, d_from, d_to, d_w);
+  return new_graph(device, n, m, 0, 1, source, out);
 }
 
 int mgb200_graph_create_rmat(int device, uint32_t scale, uint64_t edge_count, uint64_t seed, double a, double b, double c,
@@ -403,28 +380,9 @@ int mgb200_graph_create_rmat(int device, uint32_t scale, uint64_t edge_count, ui
   if (rc) return rc;
   rc = check_device(device);
   if (rc) return rc;
-  auto *h = new (std::nothrow) mgb200_graph();
-  if (!h) {
-    set_error("out of host memory");
-    return MGB200_ERR_INVALID_ARGUMENT;
-  }
-  h->g.device = device;
-  h->g.n = n;
-  h->g.m = edge_count;
-  h->g.part_rank = part_rank;
-  h->g.part_world = part_world;
   cudaSetDevice(device);
-  {
-    RmatStream source(scale, edge_count, seed, a, b, c);
-    rc = build_graph(h->g, source);
-  }
-  if (rc) {
-    free_graph(h->g);
-    delete h;
-    return rc;
-  }
-  *out = h;
-  return MGB200_OK;
+  RmatStream source(scale, edge_count, seed, a, b, c);
+  return new_graph(device, n, edge_count, part_rank, part_world, source, out);
 }
 
 }  // extern "C"
@@ -543,19 +501,14 @@ int create_from_host(int device, uint64_t n, uint64_t m, const T *from, const T 
   rc = check_device(device);
   if (rc) return rc;
   MGB_CUDA(cudaSetDevice(device));
+  DeviceBuffers coo;
   uint32_t *d_from = nullptr, *d_to = nullptr;
-  cudaError_t e;
-  if ((e = cudaMalloc(&d_from, std::max<uint64_t>(m, 1) * sizeof(uint32_t))) != cudaSuccess ||
-      (e = cudaMalloc(&d_to, std::max<uint64_t>(m, 1) * sizeof(uint32_t))) != cudaSuccess) {
-    cudaFree(d_from);
-    return cuda_fail(e, "cudaMalloc(COO)", __FILE__, __LINE__);
-  }
+  MGB_CUDA(coo.alloc(&d_from, m));
+  MGB_CUDA(coo.alloc(&d_to, m));
   const auto t0 = std::chrono::steady_clock::now();
   rc = upload_coo(device, n, m, from, to, d_from, d_to);
   const double upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   if (!rc) rc = mgb200_graph_create_device(device, n, m, d_from, d_to, part_rank, part_world, out);
-  cudaFree(d_from);
-  cudaFree(d_to);
   if (!rc) (*out)->g.upload_ms = upload_ms;
   return rc;
 }
@@ -984,22 +937,22 @@ int mgb200_hits_graph_create_host_u32(int device, uint64_t n, uint64_t m, const 
   rc = check_device(device);
   if (rc) return rc;
   MGB_CUDA(cudaSetDevice(device));
-  uint32_t *d_from = nullptr, *d_to = nullptr;
-  cudaError_t e;
-  if ((e = cudaMalloc(&d_from, std::max<uint64_t>(m, 1) * sizeof(uint32_t))) != cudaSuccess ||
-      (e = cudaMalloc(&d_to, std::max<uint64_t>(m, 1) * sizeof(uint32_t))) != cudaSuccess) {
-    cudaFree(d_from);
-    return cuda_fail(e, "cudaMalloc(COO)", __FILE__, __LINE__);
-  }
-  const auto t0 = std::chrono::steady_clock::now();
-  rc = upload_coo(device, n, m, from, to, d_from, d_to);
-  const double upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  auto *h = rc ? nullptr : new (std::nothrow) mgb200_hits_graph();
-  if (!rc && !h) {
-    set_error("out of host memory");
-    rc = MGB200_ERR_INVALID_ARGUMENT;
-  }
-  if (!rc) {
+  mgb200_hits_graph *h = nullptr;
+  double upload_ms = 0.0;
+  {  // the device COO is freed before the HITS buffers below are allocated
+    DeviceBuffers coo;
+    uint32_t *d_from = nullptr, *d_to = nullptr;
+    MGB_CUDA(coo.alloc(&d_from, m));
+    MGB_CUDA(coo.alloc(&d_to, m));
+    const auto t0 = std::chrono::steady_clock::now();
+    rc = upload_coo(device, n, m, from, to, d_from, d_to);
+    upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (rc) return rc;
+    h = new (std::nothrow) mgb200_hits_graph();
+    if (!h) {
+      set_error("out of host memory");
+      return MGB200_ERR_INVALID_ARGUMENT;
+    }
     for (Graph *g : {&h->fwd, &h->rev}) {
       g->device = device;
       g->n = n;
@@ -1014,10 +967,9 @@ int mgb200_hits_graph_create_host_u32(int device, uint64_t n, uint64_t m, const 
       rc = build_graph(h->rev, reverse);
     }
   }
-  cudaFree(d_from);
-  cudaFree(d_to);
   if (!rc) {
     h->fwd.upload_ms = upload_ms;
+    cudaError_t e;
     if ((e = cudaMalloc(&h->t_of_f, std::max<uint64_t>(n, 1) * sizeof(uint32_t))) != cudaSuccess ||
         (e = cudaMalloc(&h->f_of_t, std::max<uint64_t>(n, 1) * sizeof(uint32_t))) != cudaSuccess ||
         (e = cudaMalloc(&h->scratch, hits_scratch_doubles(n) * sizeof(double))) != cudaSuccess ||

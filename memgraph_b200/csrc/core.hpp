@@ -15,6 +15,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <string>
 #include <vector>
@@ -338,6 +339,35 @@ int cuda_fail(cudaError_t e, const char *what, const char *file, int line);
     cudaError_t _e = (expr);                                                  \
     if (_e != cudaSuccess) return ::mgb200::cuda_fail(_e, #expr, __FILE__, __LINE__); \
   } while (0)
+
+// Threads per block of the grid-stride kernels outside pagerank_kernels.cu.
+constexpr int kThreads = 256;
+
+// Grid of a grid-stride kernel over `items` threads' worth of work: one block per kThreads items, at most per_sm
+// blocks per SM, at least one block.
+inline int blocks_for(uint64_t items, int sm_count, int per_sm) {
+  const uint64_t want = (items + kThreads - 1) / kThreads;
+  return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * per_sm)));
+}
+
+// The device scratch of one call: every allocation is freed when the owner leaves its scope, on every exit path.
+struct DeviceBuffers {
+  std::vector<void *> ptrs;
+  DeviceBuffers() = default;
+  DeviceBuffers(const DeviceBuffers &) = delete;
+  DeviceBuffers &operator=(const DeviceBuffers &) = delete;
+  ~DeviceBuffers() {
+    for (void *p : ptrs) cudaFree(p);
+  }
+  template <class T>
+  cudaError_t alloc(T **out, uint64_t count) {  // max(count, 1) elements: an empty array still gets an address
+    void *p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
+    if (e == cudaSuccess) ptrs.push_back(p);
+    *out = static_cast<T *>(p);
+    return e;
+  }
+};
 
 // Where the build reads the COO from, a chunk at a time (graph_build.cu walks it twice: degrees, then the edges this
 // partition owns).  With several partitions nobody has to hold the whole edge list on a device: the transient is one

@@ -18,14 +18,6 @@
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
-
-inline int blocks_for(uint64_t items, int sm_count) {
-  const uint64_t want = (items + kThreads - 1) / kThreads;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 16;
-  return static_cast<int>(std::max<uint64_t>(1, std::min(want, cap)));
-}
-
 // ---- degrees ----------------------------------------------------------------------------------------
 
 __global__ void degree_kernel(uint64_t m, uint64_t n, const uint32_t *from, const uint32_t *to, uint32_t *outdeg,
@@ -559,32 +551,9 @@ __global__ void narrow_kernel(uint64_t count, uint64_t n, const uint64_t *in, ui
   }
 }
 
-// RAII-free scratch tracker: everything pushed here is freed when the build returns.
-struct Scratch {
-  std::vector<void *> ptrs;
-  ~Scratch() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-  void release(void *p) {
-    for (auto &q : ptrs)
-      if (q == p) {
-        cudaFree(p);
-        q = nullptr;
-      }
-  }
-};
-
 // out[0] = 0, out[i + 1] = in[0] + .. + in[i]: an exclusive scan that ends with the total
 template <typename It>
-cudaError_t prefix_sum(Scratch &tmp, It in, uint64_t *out, uint64_t count, cudaStream_t st) {
+cudaError_t prefix_sum(DeviceBuffers &tmp, It in, uint64_t *out, uint64_t count, cudaStream_t st) {
   cudaError_t e = cudaMemsetAsync(out, 0, sizeof(uint64_t), st);
   if (e != cudaSuccess || count == 0) return e;
   size_t bytes = 0;
@@ -636,7 +605,7 @@ int narrow_edges_u64_to_u32(int device, cudaStream_t stream, uint64_t n, uint64_
   if (count == 0) return MGB200_OK;
   int sm_count = 0;
   MGB_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device));
-  narrow_kernel<<<blocks_for(count, sm_count), kThreads, 0, stream>>>(count, n, d_in, d_out, d_bad_flag);
+  narrow_kernel<<<blocks_for(count, sm_count, 16), kThreads, 0, stream>>>(count, n, d_in, d_out, d_bad_flag);
   MGB_CUDA(cudaGetLastError());
   return MGB200_OK;
 }
@@ -735,7 +704,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
   g.segment_edges = env_u32("MGB200_SEGMENT_EDGES", 4096);
 
   MGB_CUDA(cudaEventRecord(g.ev[0], st));
-  Scratch tmp;
+  DeviceBuffers tmp;
   const Dealer deal{n, g.part_world};
   RowMap &map = g.map;
   map = RowMap{};
@@ -802,7 +771,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     const uint32_t *d_from = nullptr, *d_to = nullptr;
     const int grc = edges.get(first, cnt, &d_from, &d_to, st);
     if (grc) return grc;
-    degree_kernel<<<blocks_for(cnt, g.sm_count), kThreads, 0, st>>>(cnt, n, d_from, d_to, outdeg, indeg, bad);
+    degree_kernel<<<blocks_for(cnt, g.sm_count, 16), kThreads, 0, st>>>(cnt, n, d_from, d_to, outdeg, indeg, bad);
   }
   int bad_host = 0;
   MGB_CUDA(cudaMemcpyAsync(&bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -819,7 +788,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     unsigned long long *gc = nullptr;
     MGB_CUDA(tmp.alloc(&gc, 3));
     MGB_CUDA(cudaMemsetAsync(gc, 0, 3 * sizeof(unsigned long long), st));
-    class_count_kernel<<<blocks_for(n, g.sm_count), kThreads, 0, st>>>(n, indeg, g.heavy_min_degree, gc);
+    class_count_kernel<<<blocks_for(n, g.sm_count, 16), kThreads, 0, st>>>(n, indeg, g.heavy_min_degree, gc);
     unsigned long long gc_host[3] = {0, 0, 0};
     MGB_CUDA(cudaMemcpyAsync(gc_host, gc, sizeof(gc_host), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
@@ -840,7 +809,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
   MGB_CUDA(tmp.alloc(&vkey_alt, n));
   MGB_CUDA(tmp.alloc(&vid, n));
   MGB_CUDA(tmp.alloc(&vid_alt, n));
-  sort_key_kernel<<<blocks_for(n, g.sm_count), kThreads, 0, st>>>(n, indeg, outdeg, vkey, vid);
+  sort_key_kernel<<<blocks_for(n, g.sm_count, 16), kThreads, 0, st>>>(n, indeg, outdeg, vkey, vid);
   {
     cub::DoubleBuffer<uint64_t> kb(vkey, vkey_alt);
     cub::DoubleBuffer<uint32_t> vb(vid, vid_alt);
@@ -856,15 +825,15 @@ int build_graph(Graph &g, EdgeSource &edges) {
   uint32_t *indeg_l = nullptr, *vertex_of_label = nullptr;
   MGB_CUDA(tmp.alloc(&indeg_l, n));
   MGB_CUDA(tmp.alloc(&vertex_of_label, n));
-  label_kernel<<<blocks_for(n, g.sm_count), kThreads, 0, st>>>(map, vid, indeg, outdeg, g.label_of, indeg_l,
+  label_kernel<<<blocks_for(n, g.sm_count, 16), kThreads, 0, st>>>(map, vid, indeg, outdeg, g.label_of, indeg_l,
                                                               g.outdeg_l, vertex_of_label);
-  gather_local_u32_kernel<<<blocks_for(g.local_rows, g.sm_count), kThreads, 0, st>>>(g.local_rows, map, vertex_of_label,
+  gather_local_u32_kernel<<<blocks_for(g.local_rows, g.sm_count, 16), kThreads, 0, st>>>(g.local_rows, map, vertex_of_label,
                                                                                     g.local_vertex);
   const uint32_t *indeg_local = indeg_l + g.row_lo;  // dealt ranges: the owned labels are contiguous
   if (map.global_order) {
     uint32_t *gathered = nullptr;
     MGB_CUDA(tmp.alloc(&gathered, g.local_rows));
-    gather_local_u32_kernel<<<blocks_for(g.local_rows, g.sm_count), kThreads, 0, st>>>(g.local_rows, map, indeg_l,
+    gather_local_u32_kernel<<<blocks_for(g.local_rows, g.sm_count, 16), kThreads, 0, st>>>(g.local_rows, map, indeg_l,
                                                                                       gathered);
     indeg_local = gathered;
   }
@@ -879,7 +848,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
   unsigned long long *counts = nullptr;
   MGB_CUDA(tmp.alloc(&counts, 4));
   MGB_CUDA(cudaMemsetAsync(counts, 0, 4 * sizeof(unsigned long long), st));
-  class_count_kernel<<<blocks_for(g.local_rows, g.sm_count), kThreads, 0, st>>>(g.local_rows, indeg_local,
+  class_count_kernel<<<blocks_for(g.local_rows, g.sm_count, 16), kThreads, 0, st>>>(g.local_rows, indeg_local,
                                                                                g.heavy_min_degree, counts);
   unsigned long long counts_host[4] = {0, 0, 0, 0};
   MGB_CUDA(cudaMemcpyAsync(counts_host, counts, sizeof(counts_host), cudaMemcpyDeviceToHost, st));
@@ -901,7 +870,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     unsigned long long *nz = nullptr;
     MGB_CUDA(tmp.alloc(&nz, kMaxPeers));
     MGB_CUDA(cudaMemsetAsync(nz, 0, kMaxPeers * sizeof(unsigned long long), st));
-    nonzero_per_partition_kernel<<<blocks_for(n / g.part_world + 1, g.sm_count), kThreads, 0, st>>>(deal, indeg_l, nz);
+    nonzero_per_partition_kernel<<<blocks_for(n / g.part_world + 1, g.sm_count, 16), kThreads, 0, st>>>(deal, indeg_l, nz);
     unsigned long long nz_host[kMaxPeers] = {};
     MGB_CUDA(cudaMemcpyAsync(nz_host, nz, sizeof(nz_host), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
@@ -944,16 +913,16 @@ int build_graph(Graph &g, EdgeSource &edges) {
     const int grc = edges.get(first, cnt, &d_from, &d_to, st);
     if (grc) return grc;
     if (g.need_mask)
-      need_mask_kernel<<<blocks_for(cnt, g.sm_count), kThreads, 0, st>>>(cnt, d_from, d_to, g.label_of, map, g.need_mask);
+      need_mask_kernel<<<blocks_for(cnt, g.sm_count, 16), kThreads, 0, st>>>(cnt, d_from, d_to, g.label_of, map, g.need_mask);
     if (g.part_world == 1) {
-      edge_key_all_kernel<<<blocks_for(cnt, g.sm_count), kThreads, 0, st>>>(cnt, d_from, d_to, g.label_of, ekey + first);
+      edge_key_all_kernel<<<blocks_for(cnt, g.sm_count, 16), kThreads, 0, st>>>(cnt, d_from, d_to, g.label_of, ekey + first);
       if (weighted) {
         const double *d_w = edges.weights();
         MGB_CUDA(cudaMemcpyAsync(eval + first, d_w, cnt * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        out_weight_kernel<<<blocks_for(cnt, g.sm_count), kThreads, 0, st>>>(cnt, d_from, d_w, g.label_of, g.outw_l);
+        out_weight_kernel<<<blocks_for(cnt, g.sm_count, 16), kThreads, 0, st>>>(cnt, d_from, d_w, g.label_of, g.outw_l);
       }
     } else {
-      edge_key_owned_kernel<<<blocks_for(cnt, g.sm_count), kThreads, 0, st>>>(cnt, d_from, d_to, g.label_of, map, row_hi,
+      edge_key_owned_kernel<<<blocks_for(cnt, g.sm_count, 16), kThreads, 0, st>>>(cnt, d_from, d_to, g.label_of, map, row_hi,
                                                                              ekey, counts + 3);
     }
   }
@@ -1009,7 +978,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     uint64_t *block_cnt = nullptr, heavy_edges = 0;
     MGB_CUDA(tmp.alloc(&block_cnt, nh));
     MGB_CUDA(tmp.alloc(&block_ptr, nh + 1));
-    block_row_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, row_ptr, ekey, block_from, block_cnt);
+    block_row_kernel<<<blocks_for(nh, g.sm_count, 16), kThreads, 0, st>>>(nh, row_ptr, ekey, block_from, block_cnt);
     MGB_CUDA(prefix_sum(tmp, block_cnt, block_ptr, nh, st));
     MGB_CUDA(cudaMemcpyAsync(&g.block_edges, block_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaMemcpyAsync(&heavy_edges, row_ptr + nh, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -1028,7 +997,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
       MGB_CUDA(cub::DeviceSelect::If(cub_tmp, bytes, ekey, bkey, d_sel, static_cast<int64_t>(heavy_edges),
                                      BlockKey{block_from}, st));
-      block_start_kernel<<<blocks_for(ne, g.sm_count), kThreads, 0, st>>>(ne, bkey, block_ptr, block_from, block_labels,
+      block_start_kernel<<<blocks_for(ne, g.sm_count, 16), kThreads, 0, st>>>(ne, bkey, block_ptr, block_from, block_labels,
                                                                           g.tun.block_chunk, bstart);
       MGB_CUDA(prefix_sum(tmp, bstart, chunk_of, ne, st));  // chunk_of[i] = chunk of a starting edge i
       MGB_CUDA(cudaMemcpyAsync(&g.block_chunks, chunk_of + ne, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -1079,7 +1048,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       MGB_CUDA(tmp.alloc(&pair_chunk_first, pairs + 1));
       MGB_CUDA(tmp.alloc(&tile_chunks, nt));
       MGB_CUDA(cudaMemsetAsync(tile_chunks, 0, nt * sizeof(unsigned long long), st));
-      tile_pair_kernel<<<blocks_for(pairs, g.sm_count), kThreads, 0, st>>>(nh, nt, row_ptr, ekey, d_lo, d_hi,
+      tile_pair_kernel<<<blocks_for(pairs, g.sm_count, 16), kThreads, 0, st>>>(nh, nt, row_ptr, ekey, d_lo, d_hi,
                                                                           g.tun.tile_chunk, pair_cnt, pair_chunks,
                                                                           tile_chunks);
       MGB_CUDA(prefix_sum(tmp, pair_chunks, pair_chunk_first, pairs, st));
@@ -1091,7 +1060,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(tmp.alloc(&row_parts, nh));
     MGB_CUDA(tmp.alloc(&row_cold_segs, nh));
     MGB_CUDA(tmp.alloc(&cold_seg_first, nh + 1));
-    tile_row_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, nt, indeg_local, pair_cnt, pair_chunks,
+    tile_row_kernel<<<blocks_for(nh, g.sm_count, 16), kThreads, 0, st>>>(nh, nt, indeg_local, pair_cnt, pair_chunks,
                                                                     heavy_block_ptr, cold_deg, row_chunks);
     MGB_CUDA(keep_alloc(g, &g.heavy_ptr, nh + 1));
     MGB_CUDA(prefix_sum(tmp, cold_deg, g.heavy_ptr, nh, st));
@@ -1108,7 +1077,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       seg = (seg / 256) * 256;
       g.segment_edges = static_cast<uint32_t>(std::min<uint64_t>(4096, std::max<uint64_t>(256, seg)));
     }
-    seg_count_kernel<<<blocks_for(nh, g.sm_count), kThreads, 0, st>>>(nh, cold_deg, row_chunks, heavy_block_ptr, chunk_of,
+    seg_count_kernel<<<blocks_for(nh, g.sm_count, 16), kThreads, 0, st>>>(nh, cold_deg, row_chunks, heavy_block_ptr, chunk_of,
                                                                      g.segment_edges, row_parts, row_cold_segs);
     MGB_CUDA(keep_alloc(g, &g.seg_first, nh + 1));
     MGB_CUDA(prefix_sum(tmp, row_parts, g.seg_first, nh, st));
@@ -1130,7 +1099,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       cold_keys = ekey_alt;
     }
     MGB_CUDA(keep_alloc(g, &g.heavy_idx, cold_edges));
-    low32_kernel<<<blocks_for(cold_edges, g.sm_count), kThreads, 0, st>>>(cold_edges, cold_keys, idx_flags_heavy,
+    low32_kernel<<<blocks_for(cold_edges, g.sm_count, 16), kThreads, 0, st>>>(cold_edges, cold_keys, idx_flags_heavy,
                                                                          g.heavy_idx);
     if (weighted) {  // rows are sorted, heavy rows first: their weights are the prefix of the sorted weights (no tiles)
       MGB_CUDA(keep_alloc(g, &g.heavy_w, g.heavy_edges));
@@ -1142,7 +1111,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     if (g.tile_chunks || g.block_chunks) MGB_CUDA(keep_alloc(g, &g.seg_slot, g.n_cold_seg));
     MGB_CUDA(keep_alloc(g, &g.seg_partial, g.n_seg));
     MGB_CUDA(keep_alloc(g, &g.heavy_sums, nh));
-    segment_fill_kernel<<<blocks_for(nh * 32, g.sm_count), kThreads, 0, st>>>(
+    segment_fill_kernel<<<blocks_for(nh * 32, g.sm_count, 16), kThreads, 0, st>>>(
         nh, g.heavy_ptr, cold_seg_first, g.segment_edges, g.seg_first, heavy_block_ptr, chunk_of, g.seg_row, g.seg_begin,
         g.seg_slot);
     // 7c. tile chunks -> per tile, SELL-32 slices of chunks sorted by length (ties: row order)
@@ -1176,7 +1145,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       MGB_CUDA(tmp.alloc(&cbegin, nc));
       MGB_CUDA(tmp.alloc(&clen, nc));
       MGB_CUDA(tmp.alloc(&cslot, nc));
-      tile_chunk_kernel<<<blocks_for(pairs, g.sm_count), kThreads, 0, st>>>(nh, nt, row_ptr, ekey, d_lo, pair_cnt,
+      tile_chunk_kernel<<<blocks_for(pairs, g.sm_count, 16), kThreads, 0, st>>>(nh, nt, row_ptr, ekey, d_lo, pair_cnt,
                                                                            pair_chunk_first, g.seg_first,
                                                                            g.tun.tile_chunk, ckey, cid, cbegin, clen,
                                                                            cslot);
@@ -1193,7 +1162,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       }
       uint64_t *width = nullptr;
       MGB_CUDA(tmp.alloc(&width, ns));
-      tile_width_kernel<<<blocks_for(ns, g.sm_count), kThreads, 0, st>>>(ns, g.tslice_tile, g.tile_slice_first,
+      tile_width_kernel<<<blocks_for(ns, g.sm_count, 16), kThreads, 0, st>>>(ns, g.tslice_tile, g.tile_slice_first,
                                                                         d_chunk_first, sorted_id, clen, width);
       MGB_CUDA(keep_alloc(g, &g.tslice_colbase, ns + 1));
       MGB_CUDA(prefix_sum(tmp, width, g.tslice_colbase, ns, st));
@@ -1202,7 +1171,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       MGB_CUDA(cudaStreamSynchronize(st));
       MGB_CUDA(keep_alloc(g, &g.tile_idx, total_cols * kSliceRows));
       MGB_CUDA(keep_alloc(g, &g.tile_slot, ns * kSliceRows));
-      tile_fill_kernel<<<blocks_for(ns * 32, g.sm_count), kThreads, 0, st>>>(
+      tile_fill_kernel<<<blocks_for(ns * 32, g.sm_count, 16), kThreads, 0, st>>>(
           ns, g.tslice_tile, g.tile_slice_first, d_chunk_first, g.tile_base, g.tslice_colbase, sorted_id, cbegin, clen,
           cslot, ekey, static_cast<uint16_t>(T), g.tile_idx, g.tile_slot);
       // runs of heavy_tiles_kernel: contiguous slice runs of ~equal cost = columns + 8 per slice, drawn in tile order by
@@ -1223,7 +1192,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     g.n_slices = (g.n_sell + kSliceRows - 1) / kSliceRows;
     uint64_t *width = nullptr;
     MGB_CUDA(tmp.alloc(&width, g.n_slices));
-    slice_width_kernel<<<blocks_for(g.n_slices, g.sm_count), kThreads, 0, st>>>(g.n_slices, indeg_local, g.n_heavy,
+    slice_width_kernel<<<blocks_for(g.n_slices, g.sm_count, 16), kThreads, 0, st>>>(g.n_slices, indeg_local, g.n_heavy,
                                                                                width);
     MGB_CUDA(keep_alloc(g, &g.sell_colbase, g.n_slices + 1));
     {
@@ -1242,7 +1211,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     g.sell_entries = total_cols * kSliceRows;
     MGB_CUDA(keep_alloc(g, &g.sell_idx, g.sell_entries));
     if (weighted) MGB_CUDA(keep_alloc(g, &g.sell_w, g.sell_entries));
-    sell_fill_kernel<<<blocks_for(g.n_slices * 32, g.sm_count), kThreads, 0, st>>>(
+    sell_fill_kernel<<<blocks_for(g.n_slices * 32, g.sm_count, 16), kThreads, 0, st>>>(
         g.n_slices, g.n_heavy, g.n_heavy + g.n_sell, row_ptr, ekey, g.sell_colbase, static_cast<uint32_t>(n),
         idx_flags, g.sell_idx, eval, g.sell_w);
     MGB_CUDA(keep_alloc(g, &g.sell_sums, g.n_sell));
@@ -1285,9 +1254,9 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(tmp.alloc(&clen, nc));
     MGB_CUDA(tmp.alloc(&per_block, nb));
     MGB_CUDA(cudaMemsetAsync(per_block, 0, nb * sizeof(unsigned long long), st));
-    block_chunk_kernel<<<blocks_for(ne, g.sm_count), kThreads, 0, st>>>(ne, bkey, bstart, chunk_of, block_from,
+    block_chunk_kernel<<<blocks_for(ne, g.sm_count, 16), kThreads, 0, st>>>(ne, bkey, bstart, chunk_of, block_from,
                                                                         block_labels, cbegin, crow, per_block);
-    block_len_kernel<<<blocks_for(nc, g.sm_count), kThreads, 0, st>>>(nc, ne, bkey, cbegin, block_from, block_labels,
+    block_len_kernel<<<blocks_for(nc, g.sm_count, 16), kThreads, 0, st>>>(nc, ne, bkey, cbegin, block_from, block_labels,
                                                                       clen, ckey, cid);
     std::vector<unsigned long long> counts_b(nb);
     MGB_CUDA(cudaMemcpyAsync(counts_b.data(), per_block, nb * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -1329,7 +1298,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     }
     uint64_t *width = nullptr;
     MGB_CUDA(tmp.alloc(&width, ns));
-    tile_width_kernel<<<blocks_for(ns, g.sm_count), kThreads, 0, st>>>(ns, d_slice_block, d_slice_first, d_chunk_first,
+    tile_width_kernel<<<blocks_for(ns, g.sm_count, 16), kThreads, 0, st>>>(ns, d_slice_block, d_slice_first, d_chunk_first,
                                                                       sorted_id, clen, width);
     MGB_CUDA(keep_alloc(g, &g.bslice_colbase, ns + 1));
     MGB_CUDA(prefix_sum(tmp, width, g.bslice_colbase, ns, st));
@@ -1338,7 +1307,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     MGB_CUDA(cudaStreamSynchronize(st));
     MGB_CUDA(keep_alloc(g, &g.block_idx, total_cols * kSliceRows));
     MGB_CUDA(keep_alloc(g, &g.block_slot, ns * kSliceRows));
-    block_fill_kernel<<<blocks_for(ns * 32, g.sm_count), kThreads, 0, st>>>(
+    block_fill_kernel<<<blocks_for(ns * 32, g.sm_count, 16), kThreads, 0, st>>>(
         ns, d_slice_block, d_slice_first, d_chunk_first, g.bslice_colbase, sorted_id, cbegin, clen, crow, bkey, block_ptr,
         chunk_of, g.seg_first, static_cast<uint32_t>(n), g.block_idx, g.block_slot);
   }

@@ -22,10 +22,10 @@
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kPartials = 1024;
 
-inline int blocks_for(uint64_t items) {
+// one block per 4 * kThreads items, at most kPartials: the partials buffer holds one value per block
+inline int partial_blocks(uint64_t items) {
   return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>((items + kThreads * 4 - 1) / (kThreads * 4), kPartials)));
 }
 
@@ -159,8 +159,8 @@ int hits_permutations(Graph &f, Graph &t, uint32_t *t_of_f, uint32_t *f_of_t) {
   if (f.n == 0) return MGB200_OK;
   // T's build finished on T's stream; F's label arrays were final before it started
   MGB_CUDA(cudaStreamSynchronize(t.stream));
-  permutation_kernel<<<blocks_for(f.n), kThreads, 0, f.stream>>>(f.n, f.local_vertex, t.label_of, t_of_f);
-  permutation_kernel<<<blocks_for(f.n), kThreads, 0, f.stream>>>(f.n, t.local_vertex, f.label_of, f_of_t);
+  permutation_kernel<<<partial_blocks(f.n), kThreads, 0, f.stream>>>(f.n, f.local_vertex, t.label_of, t_of_f);
+  permutation_kernel<<<partial_blocks(f.n), kThreads, 0, f.stream>>>(f.n, t.local_vertex, f.label_of, f_of_t);
   MGB_CUDA(cudaGetLastError());
   MGB_CUDA(cudaStreamSynchronize(f.stream));
   return MGB200_OK;
@@ -182,7 +182,7 @@ int hits_iterate(Graph &f, Graph &t, const uint32_t *t_of_f, const uint32_t *f_o
   double *partials = scratch + n;          // [kPartials]
   double *scalars = partials + kPartials;  // [0] max auth, [1] max hubs, [2] diff, [3] spare
   double *contrib_f = f.contrib(0), *contrib_t = t.contrib(0);
-  const int blocks = blocks_for(n);
+  const int blocks = partial_blocks(n);
   uint64_t launches = 0;
   if (f.m == 0) {  // no edge: every score is 0 (the divisions by the maxima below need an edge)
     MGB_CUDA(cudaMemsetAsync(d_hubs, 0, n * sizeof(double), fs));
@@ -237,7 +237,7 @@ int hits_iterate(Graph &f, Graph &t, const uint32_t *t_of_f, const uint32_t *f_o
     launches += 4;
     sums = scalars;
   }
-  hits_write_kernel<<<blocks_for(n), kThreads, 0, fs>>>(n, t.label_of, hubs_t, contrib_t, sums, d_hubs, d_auth);
+  hits_write_kernel<<<partial_blocks(n), kThreads, 0, fs>>>(n, t.label_of, hubs_t, contrib_t, sums, d_hubs, d_auth);
   ++launches;
   MGB_CUDA(cudaEventRecord(f.ev[3], fs));
   MGB_CUDA(cudaStreamSynchronize(fs));

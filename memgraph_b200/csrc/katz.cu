@@ -18,7 +18,6 @@
 // alpha^i comes from the host's pow(), the same libm call the reference makes (:236, :244).
 #include <cmath>
 #include <cub/cub.cuh>
-#include <vector>
 
 #include "core.hpp"
 #include "katz_heap.hpp"
@@ -26,14 +25,6 @@
 
 namespace mgb200 {
 namespace {
-
-constexpr int kThreads = 256;
-
-inline int blocks_for(uint64_t items, int sm_count) {
-  const uint64_t want = (items + kThreads - 1) / kThreads;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 16;
-  return static_cast<int>(std::max<uint64_t>(1, std::min(want, cap)));
-}
 
 struct Verdict {
   unsigned int definite_fail;  // some neighbour pair violates the test under EVERY order of equal centralities
@@ -213,21 +204,6 @@ __global__ void write_by_vertex_kernel(uint64_t n, const uint32_t *label_of, con
     out[v] = c[label_of[v]];
 }
 
-struct DeviceBuffers {  // freed on every exit path
-  std::vector<void *> ptrs;
-  ~DeviceBuffers() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    const cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 struct MaxOp {
   __host__ __device__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
 };
@@ -280,7 +256,7 @@ int katz_iterate(Graph &g, double alpha, double epsilon, uint64_t max_iterations
 
   double *omega[2] = {g.contrib(0), g.contrib(1)};
   double *c = g.rank;  // one partition: local_rows == n and label == local row
-  const int grid_n = blocks_for(n, g.sm_count);
+  const int grid_n = blocks_for(n, g.sm_count, 16);
 
   MGB_CUDA(cudaEventRecord(g.ev[2], st));
   MGB_CUDA(cudaMemsetAsync(verdict, 0, sizeof(Verdict), st));
@@ -313,16 +289,16 @@ int katz_iterate(Graph &g, double alpha, double epsilon, uint64_t max_iterations
     if (rc) return rc;
     if (g.n_sell) {
       const uint64_t r0 = g.n_heavy, r1 = g.n_heavy + g.n_sell;
-      katz_sell_epilogue_kernel<<<blocks_for(r1 - r0, g.sm_count), kThreads, 0, st>>>(r0, r1, g.sell_sums, k);
+      katz_sell_epilogue_kernel<<<blocks_for(r1 - r0, g.sm_count, 16), kThreads, 0, st>>>(r0, r1, g.sell_sums, k);
       ++launches;
     }
     if (g.n_heavy) {
-      katz_heavy_finish_kernel<<<blocks_for(g.n_heavy * 32, g.sm_count), kThreads, 0, st>>>(g.n_heavy, g.seg_first,
+      katz_heavy_finish_kernel<<<blocks_for(g.n_heavy * 32, g.sm_count, 16), kThreads, 0, st>>>(g.n_heavy, g.seg_first,
                                                                                             g.seg_partial, k);
       ++launches;
     }
     if (iteration == 2 && zero_hi > zero_lo) {  // buffer 0 still holds omega_0 = 1 for the rows nobody visits
-      fill_zero_kernel<<<blocks_for(zero_hi - zero_lo, g.sm_count), kThreads, 0, st>>>(zero_lo, zero_hi, omega[0]);
+      fill_zero_kernel<<<blocks_for(zero_hi - zero_lo, g.sm_count, 16), kThreads, 0, st>>>(zero_lo, zero_hi, omega[0]);
       ++launches;
     }
     // Converged(): sort by c descending, then the neighbour tests

@@ -15,10 +15,10 @@
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kPartials = 1024;
 
-inline int blocks_for(uint64_t items) {
+// one block per 4 * kThreads items, at most kPartials: the partials buffer holds one value per block
+inline int partial_blocks(uint64_t items) {
   return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>((items + kThreads * 4 - 1) / (kThreads * 4), kPartials)));
 }
 
@@ -100,21 +100,6 @@ __global__ void __launch_bounds__(kThreads) ppr_write_kernel(uint64_t n, const u
   for (uint64_t v = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < n; v += stride) out[v] = pr[label_of[v]];
 }
 
-struct Scratch {
-  std::vector<void *> ptrs;
-  ~Scratch() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 }  // namespace
 
 int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double *d_out_original_order,
@@ -125,7 +110,7 @@ int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double 
   stats->converged = 1;
   if (n == 0) return MGB200_OK;
   cudaStream_t st = g.stream;
-  Scratch tmp;
+  DeviceBuffers tmp;
   double *pr_new = nullptr, *p = nullptr, *partials = nullptr, *scalars = nullptr;  // scalars: [0] dangling, [1] diff
   MGB_CUDA(tmp.alloc(&pr_new, n));
   MGB_CUDA(tmp.alloc(&partials, kPartials));
@@ -169,9 +154,9 @@ int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double 
   double *contrib = g.contrib(0);
   uint64_t launches = 0;
   MGB_CUDA(cudaEventRecord(g.ev[2], st));
-  ppr_init_kernel<<<blocks_for(n), kThreads, 0, st>>>(n, pr, contrib, g.state);
+  ppr_init_kernel<<<partial_blocks(n), kThreads, 0, st>>>(n, pr, contrib, g.state);
   ++launches;
-  const int blocks = blocks_for(n);
+  const int blocks = partial_blocks(n);
   uint64_t it = 0;
   int converged = 0;
   double diff_host = 0.0;
@@ -195,7 +180,7 @@ int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double 
     }
     if (it >= prm.max_iterations) break;
   }
-  ppr_write_kernel<<<blocks_for(n), kThreads, 0, st>>>(n, g.label_of, pr, d_out_original_order);
+  ppr_write_kernel<<<partial_blocks(n), kThreads, 0, st>>>(n, g.label_of, pr, d_out_original_order);
   ++launches;
   MGB_CUDA(cudaEventRecord(g.ev[3], st));
   MGB_CUDA(cudaStreamSynchronize(st));

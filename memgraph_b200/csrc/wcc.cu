@@ -36,8 +36,6 @@
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr unsigned kFull = 0xffffffffu;
 constexpr uint32_t kSampleRounds = 2;
 constexpr uint32_t kSamples = 1024;
 constexpr uint64_t kSampleSeed = 0x5eed5eed5eedull;
@@ -63,17 +61,6 @@ __device__ __forceinline__ uint32_t entry(const Lists &g, uint64_t out_begin, ui
                                           uint64_t i) {
   return i < out_deg ? g.out_adj[out_begin + i] : g.in_adj[in_begin + (i - out_deg)];
 }
-
-__device__ __forceinline__ void add_warp_sum(unsigned long long x, unsigned long long *counter) {
-  for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(kFull, x, o);
-  if ((threadIdx.x & 31) == 0 && x) atomicAdd(counter, x);
-}
-
-__device__ __forceinline__ uint64_t first_thread() { return static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; }
-__device__ __forceinline__ uint64_t thread_count() { return static_cast<uint64_t>(gridDim.x) * blockDim.x; }
-
-// Grid-stride loops below run whole warps (the bound is rounded up to a multiple of 32) so the shuffles see every lane.
-__device__ __forceinline__ uint64_t warp_rounded(uint64_t n) { return (n + 31) & ~31ull; }
 
 __global__ void __launch_bounds__(kThreads) init_kernel(uint64_t n, uint32_t *parent) {
   for (uint64_t v = first_thread(); v < n; v += thread_count()) parent[v] = static_cast<uint32_t>(v);
@@ -208,26 +195,6 @@ __global__ void __launch_bounds__(kThreads) label_kernel(uint64_t n, const uint3
   for (uint64_t v = first_thread(); v < n; v += thread_count()) component[v] = scan[parent[v]];
 }
 
-int grid_for(uint64_t threads_wanted, int sm_count, int per_sm = 8) {
-  const uint64_t want = (threads_wanted + kThreads - 1) / kThreads;
-  return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * per_sm)));
-}
-
-struct Buffers {
-  std::vector<void *> ptrs;
-  ~Buffers() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 // The most frequent value; ties go to the smaller one.
 uint32_t most_frequent(std::vector<uint32_t> values) {
   std::sort(values.begin(), values.end());
@@ -267,7 +234,7 @@ int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats
   cudaStream_t st = g->stream;
   const Lists lists{g->out_ptr, g->out_adj, g->in_ptr, g->in_adj};
 
-  Buffers buf;
+  DeviceBuffers buf;
   uint32_t *parent = nullptr, *skip = nullptr, *work = nullptr, *size = nullptr, *scan = nullptr, *roots = nullptr,
            *largest = nullptr;
   int64_t *component = nullptr;
@@ -288,7 +255,7 @@ int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats
   char *cub_tmp = nullptr;
   MGB_CUDA(buf.alloc(&cub_tmp, std::max(scan_bytes, max_bytes)));
 
-  const int grid = grid_for(n, g->sm_count);
+  const int grid = blocks_for(n, g->sm_count, 8);
   MGB_CUDA(cudaEventRecord(g->ev0, st));
   MGB_CUDA(cudaMemsetAsync(counters, 0, sizeof(Counters), st));
   MGB_CUDA(cudaMemsetAsync(size, 0, n * sizeof(uint32_t), st));
@@ -309,7 +276,7 @@ int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats
 
   mark_kernel<<<grid, kThreads, 0, st>>>(n, parent, giant, skip, counters);
   finish_kernel<<<grid, kThreads, 0, st>>>(n, lists, skip, parent, work, counters);
-  finish_warp_kernel<<<grid_for(n * 32, g->sm_count, 16), kThreads, 0, st>>>(lists, work, parent, counters);
+  finish_warp_kernel<<<blocks_for(n * 32, g->sm_count, 16), kThreads, 0, st>>>(lists, work, parent, counters);
   finish_block_kernel<<<g->sm_count * 8, kThreads, 0, st>>>(n, lists, work, parent, counters);
   compress_kernel<<<grid, kThreads, 0, st>>>(n, parent);
   stats.kernel_launches += 5;

@@ -45,9 +45,7 @@
 namespace mgb200 {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr uint32_t kSegEdges = 1024;
-constexpr unsigned kFull = 0xffffffffu;
 constexpr uint64_t kInfBits = 0x7FF0000000000000ull;
 constexpr uint64_t kUnreached = 0x7FF0000000000001ull;  // above +inf, below every NaN
 constexpr uint64_t kInvalidTag = MGB200_WSP_INVALID_TAG;
@@ -88,9 +86,6 @@ struct Counters {
   unsigned long long reached;    // produced vertices
   unsigned long long max_hops;
 };
-
-__device__ __forceinline__ uint64_t first_thread() { return static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; }
-__device__ __forceinline__ uint64_t thread_count() { return static_cast<uint64_t>(gridDim.x) * blockDim.x; }
 
 __device__ __forceinline__ uint64_t add_bits(uint64_t d, uint64_t w) {
   return static_cast<uint64_t>(__double_as_longlong(__dadd_rn(__longlong_as_double(static_cast<long long>(d)),
@@ -264,26 +259,6 @@ __global__ void output_kernel(uint64_t n, uint32_t source, const uint64_t *dist,
   }
 }
 
-int blocks_for(uint64_t items, int sm_count, int per_sm = 16) {
-  const uint64_t want = (items + kThreads - 1) / kThreads;
-  return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(want, static_cast<uint64_t>(sm_count) * per_sm)));
-}
-
-struct Buffers {
-  std::vector<void *> ptrs;
-  ~Buffers() {
-    for (void *p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T **out, uint64_t count) {
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, std::max<uint64_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(p);
-    *out = static_cast<T *>(p);
-    return e;
-  }
-};
-
 uint64_t bits_of(double x) {
   uint64_t b;
   std::memcpy(&b, &x, sizeof b);
@@ -320,7 +295,7 @@ int sort_side(mgb200_bfs_graph &g, const std::vector<uint64_t> &host_key, const 
               const uint64_t *ptr, const uint32_t *adj, double *out) {
   const uint64_t m = g.m;
   cudaStream_t st = g.stream;
-  Buffers tmp;
+  DeviceBuffers tmp;
   uint64_t *key = nullptr, *key_alt = nullptr, *val_alt = nullptr;
   int *bad = nullptr;
   uint64_t *val = reinterpret_cast<uint64_t *>(out);
@@ -341,7 +316,7 @@ int sort_side(mgb200_bfs_graph &g, const std::vector<uint64_t> &host_key, const 
   MGB_CUDA(cub::DeviceRadixSort::SortPairs(t, bytes, kb, vb, m, 0, 32 + bits, st));
   if (vb.Current() != val)
     MGB_CUDA(cudaMemcpyAsync(val, vb.Current(), m * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
-  same_pairs_kernel<<<blocks_for(m, g.sm_count), kThreads, 0, st>>>(m, g.n, kb.Current(), ptr, adj, bad);
+  same_pairs_kernel<<<blocks_for(m, g.sm_count, 16), kThreads, 0, st>>>(m, g.n, kb.Current(), ptr, adj, bad);
   MGB_CUDA(cudaGetLastError());
   int bad_host = 0;
   MGB_CUDA(cudaMemcpyAsync(&bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -463,7 +438,7 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
     if (end != s && *end == '\0' && v > 0.0 && std::isfinite(v)) delta = v;
   }
 
-  Buffers buf;
+  DeviceBuffers buf;
   uint64_t *dist = nullptr, *near_d[2] = {nullptr, nullptr};
   int32_t *hops = nullptr, *hops_dev_out = nullptr;
   uint32_t *stamp = nullptr, *bucket_stamp = nullptr, *lowered = nullptr, *near_v[2] = {nullptr, nullptr},
@@ -494,7 +469,7 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
   auto aborted = [&]() { return should_abort && should_abort(abort_user) != 0; };
   // segments + scan + relax over `nf` frontier vertices
   auto relax = [&](bool tight, uint64_t nf, const uint32_t *queue, const uint64_t *frozen, uint32_t pass) -> int {
-    segments_kernel<<<blocks_for(nf, g->sm_count), kThreads, 0, st>>>(nf, queue, adj, g->seg_count, counters);
+    segments_kernel<<<blocks_for(nf, g->sm_count, 16), kThreads, 0, st>>>(nf, queue, adj, g->seg_count, counters);
     MGB_CUDA(cub::DeviceScan::ExclusiveSum(g->cub_tmp, g->cub_tmp_bytes, g->seg_count, g->seg_scan, nf + 1, st));
     if (tight)
       relax_kernel<true><<<g->sm_count * 8, kThreads, 0, st>>>(nf, queue, frozen, g->seg_scan, adj, dist, stamp, pass,
@@ -507,7 +482,7 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
   };
 
   MGB_CUDA(cudaEventRecord(g->ev0, st));
-  init_kernel<<<blocks_for(n, g->sm_count), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), dist, hops, stamp,
+  init_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), dist, hops, stamp,
                                                                bucket_stamp, near_v[0], near_d[0], counters);
   stats.kernel_launches++;
   uint64_t nn = 1, nfar = 0;
@@ -521,7 +496,7 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
       MGB_CUDA(cudaMemsetAsync(&counters->lowered, 0, 2 * sizeof(unsigned long long), st));  // lowered, near
       int rc = relax(false, nn, near_v[cur], near_d[cur], pass);
       if (rc) return rc;
-      classify_kernel<<<blocks_for(nn * 4, g->sm_count), kThreads, 0, st>>>(
+      classify_kernel<<<blocks_for(nn * 4, g->sm_count, 16), kThreads, 0, st>>>(
           lowered, dist, T, bucket, bounded ? 1 : 0, pass, hops, bucket_stamp, near_v[cur ^ 1], near_d[cur ^ 1],
           far[fc], counters);
       stats.kernel_launches++;
@@ -535,14 +510,14 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
     if (bounded || nfar == 0) break;
     if (aborted()) return set_error("procedure aborted by the host"), MGB200_ERR_ABORTED;
     MGB_CUDA(cudaMemsetAsync(&counters->far_min, 0xff, sizeof(unsigned long long), st));
-    far_min_kernel<<<blocks_for(nfar, g->sm_count), kThreads, 0, st>>>(nfar, far[fc], dist, T, counters);
+    far_min_kernel<<<blocks_for(nfar, g->sm_count, 16), kThreads, 0, st>>>(nfar, far[fc], dist, T, counters);
     stats.kernel_launches++;
     int rc = sync_counters();
     if (rc) return rc;
     if (host.far_min == ~0ull) break;  // every far entry was handled through the near pile
     const uint64_t T_next = bucket_end(host.far_min, delta);
     MGB_CUDA(cudaMemsetAsync(&counters->near, 0, 2 * sizeof(unsigned long long), st));  // near, far
-    split_kernel<<<blocks_for(nfar, g->sm_count), kThreads, 0, st>>>(nfar, far[fc], dist, T, T_next, bucket + 1,
+    split_kernel<<<blocks_for(nfar, g->sm_count, 16), kThreads, 0, st>>>(nfar, far[fc], dist, T, T_next, bucket + 1,
                                                                      bucket_stamp, near_v[cur], near_d[cur],
                                                                      far[fc ^ 1], counters);
     stats.kernel_launches++;
@@ -577,7 +552,7 @@ int mgb200_wsp_run(mgb200_bfs_graph *g, uint64_t source, int direction, int64_t 
       q ^= 1;
     }
   }
-  output_kernel<<<blocks_for(n, g->sm_count), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), dist, hops,
+  output_kernel<<<blocks_for(n, g->sm_count, 16), kThreads, 0, st>>>(n, static_cast<uint32_t>(source), dist, hops,
                                                                  dist_dev_out, hops_dev_out, counters);
   stats.kernel_launches++;
   MGB_CUDA(cudaEventRecord(g->ev1, st));
