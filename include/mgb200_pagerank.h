@@ -72,6 +72,7 @@ typedef struct mgb200_graph_info {
   uint64_t blocks;         /* label blocks with at least one chunk (one launch each)  */
   uint64_t tile_slices;    /* SELL-32 slices of tile chunks, tile-major               */
   uint64_t tile_runs;      /* contiguous slice runs the tile kernel's CTAs draw (MGB200_TILE_RUNS) */
+  uint64_t table_labels;   /* hottest labels the SELL walk reads from shared memory (0: no table) */
 } mgb200_graph_info;
 
 typedef struct mgb200_run_stats {

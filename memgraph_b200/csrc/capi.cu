@@ -594,6 +594,7 @@ void fill_info(const Graph &g, mgb200_graph_info *info) {
   info->blocks = g.block_slice_first.empty() ? 0 : g.block_slice_first.size() - 1;
   info->tile_slices = g.tile_slices;
   info->tile_runs = g.tile_work;
+  info->table_labels = g.table_labels();
 }
 }  // namespace
 

@@ -33,6 +33,11 @@ constexpr uint32_t kIdxL1Hot = 0x40000000u;     // may allocate in L1, else bypa
 constexpr uint32_t kIdxLabelMask = 0x3FFFFFFFu; // the label itself: flagged graphs have n < 2^30
 constexpr uint32_t kNoL1Hints = 0xFFFFFFFFu;    // l1_hot_labels() when MGB200_L1_HOT_K < 0
 constexpr uint64_t kMaxBlocks = 4096;           // most label blocks (= block-pass launches per gather) of one graph
+// Shared memory the default SELL table leaves unused, so that the SM keeps L1 room for the walk's gathers in flight
+// (which land in L1 even when they do not allocate there).  On an H100 (DESIGN.md §4) the largest table, 227 KB, leaves
+// 28 KB of L1 and made the walk 16 % slower than no table at all; 195 KB (60 KB of L1) made it 11 % faster, 160 KB
+// (92 KB of L1) 12 %, 128 KB 10 %.  64 KB less than the largest is 163 KB on an H100.
+constexpr uint32_t kTableL1Room = 65536;
 
 // Which labels a partition owns and how its local rows (ascending label) map onto them.
 //   dealt ranges (default): sorted position p -> owner p % P, label = start(owner) + p / P.  Every partition owns ONE
@@ -267,7 +272,6 @@ struct Graph {
   mutable const void *occ_kernel[kOccSlots] = {};
   mutable int occ_blocks[kOccSlots] = {};
   mutable int occ_cached = 0;
-  int table_attr_bytes[2] = {0, 0};  // dynamic shared memory already granted to sell_rows_table_kernel<range / flags>
   struct Tunables {  // environment, read once per graph in build_graph()
     uint64_t l2_hot_mb = 16;     // MGB200_L2_HOT_MB: evict-last window of the gathered vector.  H100 SXM (50 MB L2, 700 W),
                                  // RMAT scale-26: 16 MB beat 8 / 24 / 32 / 48 / 64 (10.1 vs 10.2-10.8 ms per iteration)
@@ -275,7 +279,9 @@ struct Graph {
     bool multi_aware = true;     // MGB200_MULTI_AWARE=0: legacy "global label prefix is hot" on every partition
     bool force_multi_path = false;  // MGB200_FORCE_MULTI_PATH=1: run the multi-partition gather code on one GPU (measurement)
     bool stream_kernel = false;  // MGB200_SELL_KERNEL=stream
-    uint32_t smem_table_kb = 0;  // MGB200_SMEM_TABLE_KB: shared-memory hot table of the SELL kernel (0 = off)
+    long smem_table_kb = -1;     // MGB200_SMEM_TABLE_KB: shared-memory hot table of the SELL walk in KB (0 = off); unset:
+                                 // table_max_bytes - kTableL1Room, on one partition (several have not been measured)
+    uint32_t table_max_bytes = 0;  // the most dynamic shared memory the table kernel can take on this device (build_graph)
     int push_ctas = 2;           // MGB200_PUSH_CTAS: CTAs per SM of the SELL epilogue + peer push on several partitions (0 = full grid)
     int sell_mode = -1;          // MGB200_SELL_MODE: 0 ticket queue, 1 static deal, -1 (default) by partition size
     bool global_order = false;   // MGB200_LABELLING=global: label = global degree order, blocks of 32 dealt (RowMap)
@@ -295,20 +301,26 @@ struct Graph {
   // hot thresholds in LOCAL label units (label - first label of the owning partition); one definition for the
   // build-time index flags and the run-time gather window
   uint32_t hot_divisor() const { return (tun.multi_aware && !map.global_order) ? part_world : 1u; }
+  // The L1 window begins where the shared-memory table ends: a table label is never gathered from global memory, so a
+  // window that started at label 0 would lie (partly or wholly) inside the table and allocate nothing
   uint32_t l1_hot_labels() const {
     if (tun.l1_hot_k < 0) return kNoL1Hints;
-    const uint64_t v = static_cast<uint64_t>(tun.l1_hot_k) * 1024 / hot_divisor();
+    const uint64_t v = table_labels() / part_world + static_cast<uint64_t>(tun.l1_hot_k) * 1024 / hot_divisor();
     return static_cast<uint32_t>(v < 0xFFFFFFF0ull ? v : 0xFFFFFFF0ull);
   }
   // labels in the shared-memory hot table: a multiple of 2 * partitions (every owner's window has an even size, a whole
   // number of 16-byte TMA units on one partition); only with 30-bit labels on several partitions (the slot rides in
-  // the stored index), never with the per-gather owner lookup
+  // the stored index), never with the per-gather owner lookup.  On by default on one partition only.
   uint32_t table_labels() const {
     if (tun.smem_table_kb == 0 || tun.stream_kernel) return 0;
+    if (tun.smem_table_kb < 0 && part_world > 1) return 0;
     if (part_world > 1 && (!idx_flagged || map.global_order)) return 0;
     if (part_world == 1 && (idx_flagged || tun.force_multi_path)) return 0;
     const uint64_t unit = 2ull * part_world;
-    uint64_t labels = std::min<uint64_t>(static_cast<uint64_t>(tun.smem_table_kb) * 1024 / sizeof(double), n);
+    const uint64_t bytes = tun.smem_table_kb < 0 ? (tun.table_max_bytes > kTableL1Room ? tun.table_max_bytes - kTableL1Room : 0)
+                                                 : std::min<uint64_t>(static_cast<uint64_t>(tun.smem_table_kb) * 1024,
+                                                                      tun.table_max_bytes);
+    uint64_t labels = std::min<uint64_t>(bytes / sizeof(double), n);
     labels = labels / unit * unit;
     return static_cast<uint32_t>(labels);
   }
@@ -405,6 +417,11 @@ int launch_barrier(Graph &g);
 int launch_sum_and_exchange(Graph &g);
 int launch_write_ranks_original_order(Graph &g, double *d_out);                   // single partition
 int launch_write_ranks_local(Graph &g, double *d_rank_out, uint32_t *d_vertex_out);  // partitioned
+// the most dynamic shared memory the SELL table kernel can take on `device` (opt-in shared memory per block minus the
+// kernel's static shared memory, in whole 16-byte TMA units), granted to the kernel on the current device
+int setup_sell_table_kernel(int device, uint32_t *bytes);
+// warps per SM of the SELL kernel that this graph's unweighted gathers launch (the basis of its work items)
+int sell_warps_per_sm(const Graph &g);
 
 // katz.cu
 struct KatzResult {

@@ -677,7 +677,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     if ((s = getenv("MGB200_IDX_FLAGS")) != nullptr) g.tun.idx_flags = atoi(s);
     if ((s = getenv("MGB200_SELL_MODE")) != nullptr) g.tun.sell_mode = atoi(s);
     if ((s = getenv("MGB200_PUSH_CTAS")) != nullptr) g.tun.push_ctas = std::max(0, atoi(s));
-    if ((s = getenv("MGB200_SMEM_TABLE_KB")) != nullptr) g.tun.smem_table_kb = static_cast<uint32_t>(std::min(224, std::max(0, atoi(s))));
+    if ((s = getenv("MGB200_SMEM_TABLE_KB")) != nullptr) g.tun.smem_table_kb = std::max(0l, strtol(s, nullptr, 10));
     if ((s = getenv("MGB200_LABELLING")) != nullptr) g.tun.global_order = strcmp(s, "global") == 0;
     if ((s = getenv("MGB200_PUSH_MASK")) != nullptr) g.tun.push_mask = s[0] == '1';
     if ((s = getenv("MGB200_LONE_PARTITION")) != nullptr) g.tun.lone_partition = s[0] == '1';
@@ -693,6 +693,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
       if (ms) g.tun.barrier_timeout_ms = ms;
     }
   }
+  if (const int rc = setup_sell_table_kernel(g.device, &g.tun.table_max_bytes)) return rc;
   if (edges.weighted()) {  // weighted gathers exist on the range path only: the knobs that leave it do not apply
     g.tun.idx_flags = 0;
     g.tun.force_multi_path = false;
@@ -1224,8 +1225,9 @@ int build_graph(Graph &g, EdgeSource &edges) {
     // graph); below that every extra run start costs more than the balance gains and ONE (or two) contiguous runs per
     // warp, dealt statically, are faster (the partitions of a multi-GPU run).
     const uint64_t kSliceCost = env_u32_zero("MGB200_SLICE_COST", 8);
-    const uint64_t resident_warps = static_cast<uint64_t>(g.sm_count) * 32u;  // item basis: 32 warps per SM (the
-                                                                               // kernel holds 3 CTAs x 8 warps)
+    // item basis: the warps resident at once in the kernel that will walk them (24 per SM for the plain and the table
+    // walk); a deal sized for more warps than run gives some warps one item more than the rest
+    const uint64_t resident_warps = static_cast<uint64_t>(g.sm_count) * sell_warps_per_sm(g);
     const uint64_t per_warp = g.n_slices / resident_warps;
     g.sell_static = g.tun.sell_mode >= 0 ? g.tun.sell_mode == 1 : per_warp < 64;
     const uint64_t items_default = !g.sell_static ? resident_warps * 16 : (per_warp < 32 ? resident_warps : resident_warps * 2);

@@ -539,11 +539,15 @@ __global__ void __launch_bounds__(kBlockThreads, MGB_SELL_MIN_BLOCKS) sell_rows_
   sell_walk<kPathRange, false, true>(a, nullptr);
 }
 
-// The same walk with the hot table: ONE 1024-thread CTA per SM (32 warps, at most 64 registers each) so that the SM
-// holds one copy of the table; filled once per launch -- one partition: TMA bulk copies (cp.async.bulk, 32 KiB each,
-// completion on an mbarrier, L2 evict-last) of the contiguous label prefix; several partitions: one window per owner,
-// whose first label is only 8-byte aligned, so the threads load it cooperatively.
-constexpr int kTableThreads = 1024;
+// The same walk with the hot table: ONE CTA per SM so that the SM holds one copy of the table; filled once per launch --
+// one partition: TMA bulk copies (cp.async.bulk, 32 KiB each, completion on an mbarrier, L2 evict-last) of the
+// contiguous label prefix; several partitions: one window per owner, whose first label is only 8-byte aligned, so the
+// threads load it cooperatively.  768 threads = the plain kernel's 24 warps per SM, with up to 85 registers each: at
+// 1024 threads ptxas caps the walk at 64 registers and it spills, as the plain walk did at 4 CTAs per SM (DESIGN.md §4).
+#ifndef MGB_TABLE_THREADS
+#define MGB_TABLE_THREADS 768
+#endif
+constexpr int kTableThreads = MGB_TABLE_THREADS;
 template <int kPath>
 __global__ void __launch_bounds__(kTableThreads, 1) sell_rows_table_kernel(const SellArgs a) {
   extern __shared__ __align__(128) unsigned char table_smem[];
@@ -1216,7 +1220,44 @@ double zero_row_rank(const Graph &g, const IterateConfig &cfg) {
   return cfg.max_iterations == 0 ? 1.0 / static_cast<double>(g.n) : (1.0 - cfg.damping) / static_cast<double>(g.n);
 }
 
-// SELL rows: the plain kernel (MGB_SELL_MIN_BLOCKS x 256 threads per SM) or, with a hot table, one 1024-thread CTA per SM
+using SellKernel = void (*)(SellArgs);
+static SellKernel plain_sell_kernel(uint32_t path) {
+  return path == kPathFlags ? sell_rows_kernel<kPathFlags>
+         : path == kPathLookup ? sell_rows_kernel<kPathLookup>
+                               : sell_rows_kernel<kPathRange>;
+}
+
+int setup_sell_table_kernel(int device, uint32_t *bytes) {
+  int optin = 0;
+  MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+  const void *const kernels[] = {reinterpret_cast<const void *>(sell_rows_table_kernel<kPathRange>),
+                                 reinterpret_cast<const void *>(sell_rows_table_kernel<kPathFlags>)};
+  size_t static_bytes = 0;
+  for (const void *fn : kernels) {
+    cudaFuncAttributes attr{};
+    MGB_CUDA(cudaFuncGetAttributes(&attr, fn));
+    static_bytes = std::max(static_bytes, attr.sharedSizeBytes);
+  }
+  const size_t room = static_cast<size_t>(optin) > static_bytes ? static_cast<size_t>(optin) - static_bytes : 0;
+  *bytes = static_cast<uint32_t>(room / 16 * 16);
+  // The dynamic shared memory limit is a property of the kernel on the device, shared by every graph handle of the
+  // process: it is always raised to the device's largest table, never set to one handle's table size, which a
+  // concurrent call with a larger table would then exceed at launch.  The carveout hint keeps the L1 / shared split at
+  // the smallest shared part each launch's table needs (the L1 left over is what the walk's gathers land in).
+  for (const void *fn : kernels) {
+    MGB_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(*bytes)));
+    MGB_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
+  }
+  return MGB200_OK;
+}
+
+int sell_warps_per_sm(const Graph &g) {
+  const GatherWindow w = make_window(g);
+  if (w.table_n > 0 && w.path != kPathLookup) return kTableThreads / 32;
+  return grid_for(g, reinterpret_cast<const void *>(plain_sell_kernel(w.path))) / g.sm_count * kWarpsPerBlock;
+}
+
+// SELL rows: the plain kernel (MGB_SELL_MIN_BLOCKS x 256 threads per SM) or, with a hot table, one kTableThreads CTA per SM
 int launch_sell_rows(Graph &g, const SellArgs &s) {
   const uint32_t table_n = s.window.table_n;
   if (s.w != nullptr) {
@@ -1230,17 +1271,11 @@ int launch_sell_rows(Graph &g, const SellArgs &s) {
     sell_rows_weighted_kernel<<<grid, kBlockThreads, 0, g.stream>>>(s);
   } else if (table_n > 0 && s.window.path != kPathLookup) {
     void (*const fn)(SellArgs) = s.window.path == kPathFlags ? sell_rows_table_kernel<kPathFlags> : sell_rows_table_kernel<kPathRange>;
-    const int bytes = static_cast<int>(table_n * sizeof(double));
-    if (g.table_attr_bytes[s.window.path == kPathFlags] < bytes) {
-      MGB_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-      g.table_attr_bytes[s.window.path == kPathFlags] = bytes;
-    }
+    const int bytes = static_cast<int>(table_n * sizeof(double));  // <= the limit setup_sell_table_kernel granted
     const int grid = static_cast<int>(std::min<uint64_t>(g.sm_count, ceil_div(g.sell_work, kTableThreads / 32)));
     fn<<<grid, kTableThreads, bytes, g.stream>>>(s);
   } else {
-    void (*const sell_fn)(SellArgs) = s.window.path == kPathFlags    ? sell_rows_kernel<kPathFlags>
-                                      : s.window.path == kPathLookup ? sell_rows_kernel<kPathLookup>
-                                                                     : sell_rows_kernel<kPathRange>;
+    const SellKernel sell_fn = plain_sell_kernel(s.window.path);
     const int grid = static_cast<int>(std::min(
         static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(sell_fn))), ceil_div(g.sell_work, kWarpsPerBlock)));
     sell_fn<<<grid, kBlockThreads, 0, g.stream>>>(s);

@@ -21,6 +21,10 @@ VARIANTS = {
     "s_b4": ["-DMGB_SELL_MIN_BLOCKS=4"], "s_b3": ["-DMGB_SELL_MIN_BLOCKS=3"], "s_u6": ["-DMGB_SELL_UNROLL=6", "-DMGB_SELL_MIN_BLOCKS=4"],
     "s_u4": ["-DMGB_SELL_UNROLL=4", "-DMGB_SELL_MIN_BLOCKS=4"],
     "s_u12b3": ["-DMGB_SELL_UNROLL=12", "-DMGB_SELL_MIN_BLOCKS=3"], "s_u16b2": ["-DMGB_SELL_UNROLL=16", "-DMGB_SELL_MIN_BLOCKS=2"],
+    # SELL table kernel threads (one CTA per SM): 1024 caps it at 64 registers and spills, 768 does not; and the walk's
+    # unroll at 768 threads (MGB_SELL_UNROLL also sets the plain kernel's)
+    "t1024": ["-DMGB_TABLE_THREADS=1024"], "t768": ["-DMGB_TABLE_THREADS=768"],
+    "t768_u6": ["-DMGB_TABLE_THREADS=768", "-DMGB_SELL_UNROLL=6"], "t768_u12": ["-DMGB_TABLE_THREADS=768", "-DMGB_SELL_UNROLL=12"],
 }
 
 
@@ -39,8 +43,9 @@ def main():
             raise SystemExit(1)
         sell = ""
         lines = log.stdout.splitlines()
-        for i, l in enumerate(lines):  # registers and spills of the SELL walk and the heavy-segment kernel
-            if "Compiling entry function" in l and ("sell_rows_kernelILi0E" in l or "heavy_segments_kernelILi0ELb0E" in l):
+        for i, l in enumerate(lines):  # registers and spills of the SELL walks (plain, table) and the heavy-segment kernel
+            if "Compiling entry function" in l and ("sell_rows_kernelILi0E" in l or "sell_rows_table_kernelILi0E" in l or
+                                                    "heavy_segments_kernelILi0ELb0E" in l):
                 sell += " | ".join(x.strip() for x in lines[i + 2:i + 4]) + "\n           "
         subprocess.run([B.NVCC, "-shared", "-cudart", "static", "-o", os.path.join(out, "libmgb200_pagerank.so"), obj] + others, check=True)
         print(f"{name:10s} {sell.rstrip()}")
