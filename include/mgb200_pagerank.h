@@ -73,6 +73,7 @@ typedef struct mgb200_graph_info {
   uint64_t tile_slices;    /* SELL-32 slices of tile chunks, tile-major               */
   uint64_t tile_runs;      /* contiguous slice runs the tile kernel's CTAs draw (MGB200_TILE_RUNS) */
   uint64_t table_labels;   /* hottest labels the SELL walk reads from shared memory (0: no table) */
+  uint64_t stage_entries;  /* SELL entries read from values the block passes stage (MGB200_SELL_STAGE) */
 } mgb200_graph_info;
 
 typedef struct mgb200_run_stats {

@@ -20,7 +20,8 @@ class GraphInfo(ctypes.Structure):
                 ("zero_rows", u64), ("resident_bytes", u64), ("build_ms", f64), ("upload_ms", f64), ("build_peak_bytes", u64),
                 ("tiled_edges", u64), ("tile_chunks", u64),
                 ("block_edges", u64), ("block_chunks", u64), ("blocks", u64),
-                ("tile_slices", u64), ("tile_runs", u64), ("table_labels", u64)]
+                ("tile_slices", u64), ("tile_runs", u64), ("table_labels", u64),
+                ("stage_entries", u64)]
 
 
 class RunStatsC(ctypes.Structure):

@@ -595,6 +595,7 @@ void fill_info(const Graph &g, mgb200_graph_info *info) {
   info->tile_slices = g.tile_slices;
   info->tile_runs = g.tile_work;
   info->table_labels = g.table_labels();
+  info->stage_entries = g.stage_entries;
 }
 }  // namespace
 

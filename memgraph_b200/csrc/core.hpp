@@ -31,6 +31,8 @@ constexpr uint32_t kMaxTileLabels = 28672;  // (T + 1) doubles of shared memory 
 constexpr uint32_t kIdxL2Hot = 0x80000000u;     // keep in L2 (evict_last), else evict_first
 constexpr uint32_t kIdxL1Hot = 0x40000000u;     // may allocate in L1, else bypass
 constexpr uint32_t kIdxLabelMask = 0x3FFFFFFFu; // the label itself: flagged graphs have n < 2^30
+// On one partition without flags, bit 31 of a SELL index marks a staged entry: the rest is its slot in stage_val
+constexpr uint32_t kIdxStaged = 0x80000000u;
 constexpr uint32_t kNoL1Hints = 0xFFFFFFFFu;    // l1_hot_labels() when MGB200_L1_HOT_K < 0
 constexpr uint64_t kMaxBlocks = 4096;           // most label blocks (= block-pass launches per gather) of one graph
 // Shared memory the default SELL table leaves unused, so that the SM keeps L1 room for the walk's gathers in flight
@@ -219,6 +221,13 @@ struct Graph {
   uint64_t *bslice_colbase = nullptr;       // [block_slices + 1] in units of 32-entry columns
   uint32_t *block_idx = nullptr;            // [32 * columns] source labels, pad = n
   uint64_t *block_slot = nullptr;           // [32 * block_slices] partial written by each lane; ~0 = padding lane
+  // SELL staging (graph_build.cu step 10): a SELL entry whose source lies in a launched block is read by the walk from
+  // stage_val, which that block's pass fills (stage_val[q] = vec[stage_src[q]]) while the block sits in L2.  Slots are
+  // ordered by (block, position in sell_idx), so a column's lanes read neighbouring slots.
+  uint64_t stage_entries = 0;
+  std::vector<uint64_t> stage_first;  // host: [launched blocks + 1] first slot of every block's pass
+  uint32_t *stage_src = nullptr;      // [stage_entries] source label of every slot
+  double *stage_val = nullptr;        // [stage_entries] its value in the vector the current gather reads
   double *heavy_sums = nullptr;   // [n_heavy] per-row gathered sums of the current iteration
   // optional edge weights (cuGraph-semantics variants only; one partition): parallel to heavy_idx / sell_idx, pad = 0
   double *heavy_w = nullptr, *sell_w = nullptr;
@@ -228,7 +237,8 @@ struct Graph {
   uint64_t n_slices = 0;
   uint64_t sell_entries = 0;
   uint64_t *sell_colbase = nullptr;  // [n_slices + 1] in units of 32-entry columns
-  uint32_t *sell_idx = nullptr;      // [sell_entries] source labels (+ hot flags if idx_flagged), pad = n
+  uint32_t *sell_idx = nullptr;      // [sell_entries] source labels (+ hot flags if idx_flagged; kIdxStaged | slot for a
+                                     // staged entry), pad = n
   bool idx_flagged = false;          // bits 31/30 of every stored index = L2-hot / L1-hot (graph_build.cu IndexFlags)
   double *sell_sums = nullptr;       // [n_sell] per-row gathered sums of the current iteration
   uint32_t sell_items = 0;           // work items of the streaming kernel: contiguous slice runs, ~equal columns
@@ -296,6 +306,8 @@ struct Graph {
     uint64_t block_labels = 2u << 20;  // MGB200_BLOCK_LABELS: labels per block (0 = off)
     uint32_t block_chunk = 16;         // MGB200_BLOCK_CHUNK: most edges of one block chunk (DESIGN.md §4: a pass lasts
                                        // as long as its longest chunk's chain of dependent gathers)
+    int sell_stage = -1;               // MGB200_SELL_STAGE: 1 stage, 0 never, -1 (default) when the gathered vector is
+                                       // larger than the device's L2 (graph_build.cu step 10)
     unsigned long long barrier_timeout_ms = 20000;  // MGB200_BARRIER_TIMEOUT_MS
   } tun;
   // hot thresholds in LOCAL label units (label - first label of the owning partition); one definition for the

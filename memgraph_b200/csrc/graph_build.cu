@@ -502,6 +502,42 @@ __global__ void block_fill_kernel(uint64_t n_slices, const uint32_t *slice_block
   }
 }
 
+// ---- SELL staging ----------------------------------------------------------------------------------------------
+
+// Key of SELL entry i: (launch index of its source's block << kStagePosBits) | i when the source lies in a block that
+// has a pass, else ~0 (the entry keeps its label: sources below block_from, the pad slot n, blocks without a pass)
+constexpr int kStagePosBits = 40;
+struct StageKey {
+  const uint32_t *idx;       // sell_idx, plain labels
+  const uint32_t *launched;  // [blocks] launch index of every label block, ~0 = no pass
+  uint64_t from, labels, n;
+  __device__ uint64_t operator()(uint64_t i) const {
+    const uint32_t l = idx[i];
+    if (l < from || l >= n) return ~0ull;
+    const uint32_t j = launched[(l - from) / labels];
+    return j == ~0u ? ~0ull : (static_cast<uint64_t>(j) << kStagePosBits) | i;
+  }
+};
+struct IsStaged {  // predicate and 0/1 count of a StageKey
+  __device__ uint64_t operator()(uint64_t key) const { return key != ~0ull; }
+};
+
+// slot q = rank of its key in (block, position) order: stage_src[q] = the entry's label, the entry becomes the slot
+__global__ void stage_fill_kernel(uint64_t count, const uint64_t *key, uint32_t *sell_idx, uint32_t *stage_src) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t q = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; q < count; q += stride) {
+    const uint64_t i = key[q] & ((1ull << kStagePosBits) - 1);
+    stage_src[q] = sell_idx[i];
+    sell_idx[i] = kIdxStaged | static_cast<uint32_t>(q);
+  }
+}
+
+// first[j] = first slot of launched block j (j <= blocks: first[blocks] = count)
+__global__ void stage_first_kernel(uint32_t blocks, uint64_t count, const uint64_t *key, uint64_t *first) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j <= blocks) first[j] = lower_bound_key(key, 0, count, static_cast<uint64_t>(j) << kStagePosBits);
+}
+
 // work items for the streaming SELL kernel: item i starts at the first slice whose column base is
 // >= i * total_cols / n_items (binary search over the slice column bases)
 __global__ void sell_items_kernel(uint32_t n_items, uint64_t n_slices, const uint64_t *colbase, uint64_t total_cols,
@@ -627,7 +663,7 @@ void free_graph(Graph &g) {
   if (g.outw_l) cudaFree(g.outw_l);
   void *tile_ptrs[] = {g.seg_slot,  g.tile_base, g.tile_load, g.tile_slice_first, g.tslice_tile,
                        g.tslice_colbase, g.tile_idx, g.tile_slot, g.tile_work_begin, g.bslice_colbase, g.block_idx,
-                       g.block_slot};
+                       g.block_slot, g.stage_src, g.stage_val};
   for (void *p : tile_ptrs)
     if (p) cudaFree(p);
   void *ptrs[] = {g.label_of,  g.outdeg_l,  g.local_vertex, g.heavy_ptr,    g.heavy_idx, g.seg_row,     g.seg_begin,
@@ -688,6 +724,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
     if ((s = getenv("MGB200_BLOCK_FROM")) != nullptr) g.tun.block_from = std::min<uint64_t>(strtoull(s, nullptr, 10), ~0u);
     if ((s = getenv("MGB200_BLOCK_LABELS")) != nullptr) g.tun.block_labels = strtoull(s, nullptr, 10);
     g.tun.block_chunk = env_u32("MGB200_BLOCK_CHUNK", g.tun.block_chunk);
+    if ((s = getenv("MGB200_SELL_STAGE")) != nullptr) g.tun.sell_stage = s[0] == '1' ? 1 : 0;
     if ((s = getenv("MGB200_BARRIER_TIMEOUT_MS")) != nullptr) {
       const unsigned long long ms = strtoull(s, nullptr, 10);
       if (ms) g.tun.barrier_timeout_ms = ms;
@@ -1242,6 +1279,7 @@ int build_graph(Graph &g, EdgeSource &edges) {
   }
 
   // 9. block chunks -> per block, SELL-32 slices of chunks sorted by length (ties: row order); empty blocks are skipped
+  std::vector<uint32_t> launched_of;  // [blocks] launch index of every label block, ~0 = empty (no pass)
   if (g.block_chunks) {
     const uint64_t nb = (n - block_from + block_labels - 1) / block_labels, nc = g.block_chunks, ne = g.block_edges;
     uint64_t *cbegin = nullptr, *ckey = nullptr, *ckey_alt = nullptr, *cid = nullptr, *cid_alt = nullptr;
@@ -1267,12 +1305,14 @@ int build_graph(Graph &g, EdgeSource &edges) {
     std::vector<uint32_t> slice_block;
     g.block_slice_first.assign(1, 0);
     g.block_lo.clear();
+    launched_of.assign(nb, ~0u);
     for (uint64_t b = 0; b < nb; ++b) {
       chunk_first[b + 1] = chunk_first[b] + counts_b[b];
       const uint64_t slices = (counts_b[b] + kSliceRows - 1) / kSliceRows;
       slice_first[b + 1] = slice_first[b] + slices;
       slice_block.insert(slice_block.end(), slices, static_cast<uint32_t>(b));
       if (slices) {
+        launched_of[b] = static_cast<uint32_t>(g.block_lo.size());
         g.block_slice_first.push_back(slice_first[b + 1]);
         g.block_lo.push_back(static_cast<uint32_t>(block_from + b * block_labels));
       }
@@ -1312,6 +1352,65 @@ int build_graph(Graph &g, EdgeSource &edges) {
     block_fill_kernel<<<blocks_for(ns * 32, g.sm_count, 16), kThreads, 0, st>>>(
         ns, d_slice_block, d_slice_first, d_chunk_first, g.bslice_colbase, sorted_id, cbegin, clen, crow, bkey, block_ptr,
         chunk_of, g.seg_first, static_cast<uint32_t>(n), g.block_idx, g.block_slot);
+  }
+
+  // 10. SELL staging: the SELL entries whose source lies in a block with a pass become slots of stage_val, which that
+  // pass fills while the block is in L2, so the walk reads them in slot order instead of one random HBM sector each.
+  // The slots are ordered by (block, position in sell_idx); sell_idx is column-major per slice, so a column's lanes
+  // read neighbouring slots.  Bit 31 marks a slot: plain labels only (no hot flags), n < 2^31, fewer than 2^31 slots;
+  // the stream kernel reads raw labels.  The add order inside a row does not change.  By default only where the vector
+  // is larger than L2: where it fits, the walk's gathers from the blocks hit L2 anyway and the copy is pure cost (RMAT-22
+  // Katz, 32 MB on an H100's 50 MB L2: 1.4 % slower per iteration with staging, DESIGN.md §4).
+  const bool stage_wanted = g.tun.sell_stage > 0 ||
+                            (g.tun.sell_stage < 0 && (n + 1) * sizeof(double) > static_cast<uint64_t>(prop.l2CacheSize));
+  const bool stage_on = stage_wanted && !launched_of.empty() && g.sell_entries > 0 && !g.idx_flagged &&
+                        !g.tun.stream_kernel && n < (1ull << 31) && g.sell_entries < (1ull << kStagePosBits);
+  if (stage_on) {
+    const uint64_t ent = g.sell_entries;
+    const uint32_t nl = static_cast<uint32_t>(g.block_lo.size());
+    uint32_t *d_launched = nullptr;
+    MGB_CUDA(tmp.alloc(&d_launched, launched_of.size()));
+    MGB_CUDA(cudaMemcpyAsync(d_launched, launched_of.data(), launched_of.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    const StageKey stage_key{g.sell_idx, d_launched, block_from, block_labels, n};
+    cub::TransformInputIterator<uint64_t, StageKey, cub::CountingInputIterator<uint64_t>> keys_in(
+        cub::CountingInputIterator<uint64_t>(0), stage_key);
+    cub::TransformInputIterator<uint64_t, IsStaged, decltype(keys_in)> staged_in(keys_in, IsStaged{});
+    unsigned long long *d_count = nullptr;
+    MGB_CUDA(tmp.alloc(&d_count, 1));
+    size_t bytes = 0;
+    void *cub_tmp = nullptr;
+    MGB_CUDA(cub::DeviceReduce::Sum(nullptr, bytes, staged_in, d_count, static_cast<int64_t>(ent), st));
+    MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+    MGB_CUDA(cub::DeviceReduce::Sum(cub_tmp, bytes, staged_in, d_count, static_cast<int64_t>(ent), st));
+    unsigned long long count = 0;
+    MGB_CUDA(cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaStreamSynchronize(st));
+    if (count > 0 && count < (1ull << 31)) {  // else the entries keep their labels
+      uint64_t *skey = nullptr, *skey_alt = nullptr;
+      MGB_CUDA(tmp.alloc(&skey, count));
+      MGB_CUDA(tmp.alloc(&skey_alt, count));
+      bytes = 0;
+      MGB_CUDA(cub::DeviceSelect::If(nullptr, bytes, keys_in, skey, d_count, static_cast<int64_t>(ent), IsStaged{}, st));
+      MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+      MGB_CUDA(cub::DeviceSelect::If(cub_tmp, bytes, keys_in, skey, d_count, static_cast<int64_t>(ent), IsStaged{}, st));
+      // positions ascend already: a stable sort on the block bits alone gives (block, position) order
+      cub::DoubleBuffer<uint64_t> kb(skey, skey_alt);
+      bytes = 0;
+      const int end_bit = kStagePosBits + bits_for(nl);
+      MGB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, kb, count, kStagePosBits, end_bit, st));
+      MGB_CUDA(tmp.alloc(reinterpret_cast<char **>(&cub_tmp), bytes));
+      MGB_CUDA(cub::DeviceRadixSort::SortKeys(cub_tmp, bytes, kb, count, kStagePosBits, end_bit, st));
+      MGB_CUDA(keep_alloc(g, &g.stage_src, count));
+      MGB_CUDA(keep_alloc(g, &g.stage_val, count));
+      stage_fill_kernel<<<blocks_for(count, g.sm_count, 16), kThreads, 0, st>>>(count, kb.Current(), g.sell_idx, g.stage_src);
+      uint64_t *d_first = nullptr;
+      MGB_CUDA(tmp.alloc(&d_first, nl + 1));
+      stage_first_kernel<<<(nl + 1 + kThreads - 1) / kThreads, kThreads, 0, st>>>(nl, count, kb.Current(), d_first);
+      g.stage_first.resize(nl + 1);
+      MGB_CUDA(cudaMemcpyAsync(g.stage_first.data(), d_first, (nl + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+      MGB_CUDA(cudaStreamSynchronize(st));
+      g.stage_entries = count;
+    }
   }
   note_mem(g);
   MGB_CUDA(cudaGetLastError());

@@ -117,15 +117,31 @@ __device__ __forceinline__ GatherPolicy make_gather_policy(const double *contrib
 // and the degree-sorted labelling makes "hottest" a prefix -- 21 % of all gathers of RMAT-26 go to the first 16 K
 // labels, 27 % to the first 28 K (scripts/topk_share.py).  One partition: slot = label (label < table_n).  Several
 // partitions: the build stored the slot in the index itself, code 01 in bits 31/30 (graph_build.cu IndexFlags).
-template <int kPath, bool kSelectL2 = true, bool kTable = false>
+// kStaged (the SELL walk on the range path): an index with kIdxStaged set is a slot of `staged` (graph_build.cu step 10),
+// filled by the block pass of its source's block; it is read once per gather, evict-first in L2.
+#ifndef MGB_STAGE_L1
+#define MGB_STAGE_L1 1  // staged reads: 1 default L1 allocation (neighbouring columns share sectors), 0 no_allocate
+#endif
+template <int kPath, bool kSelectL2 = true, bool kTable = false, bool kStaged = false>
 __device__ __forceinline__ double ld_contrib_at(const double *base, uint32_t src, const GatherPolicy &gp,
-                                                const GatherWindow &w, const double *table = nullptr) {
+                                                const GatherWindow &w, const double *table = nullptr,
+                                                const double *staged = nullptr) {
   if (kTable) {
     if (kPath == kPathFlags) {
       if ((src >> 30) == 1u) return table[src & kIdxLabelMask];
     } else if (src < w.table_n) {
       return table[src];
     }
+  }
+  if (kStaged && kPath == kPathRange && (src & kIdxStaged)) {
+    const double *p = staged + (src & ~kIdxStaged);
+    double v;
+#if MGB_STAGE_L1
+    asm volatile("ld.global.nc.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(gp.cold));
+#else
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(gp.cold));
+#endif
+    return v;
   }
   uint32_t label = src;
   uint64_t pol = gp.hot;
@@ -398,6 +414,7 @@ struct SellArgs {
   GatherWindow window;
   IterState *state;
   double *sums;  // [n_sell] per-row sums of gathered contributions (consumed by row_epilogue_kernel)
+  const double *stage_val;  // staged values of the entries marked kIdxStaged (filled by the block passes), or nullptr
 };
 
 // Tunables (compile-time; variants: scripts/build_variants.py)
@@ -485,7 +502,8 @@ __device__ __forceinline__ void sell_walk(const SellArgs &a, const double *table
       }
 #pragma unroll
       for (int j = 0; j < kSellUnroll; ++j)
-        if (k + j < ncols) v[j] = ld_contrib_at<kPath, true, kTable>(a.contrib_in, src[j], gpol, a.window, table);
+        if (k + j < ncols)
+          v[j] = ld_contrib_at<kPath, true, kTable, !kWeighted>(a.contrib_in, src[j], gpol, a.window, table, a.stage_val);
       if (kWeighted) {
 #pragma unroll
         for (int j = 0; j < kSellUnroll; ++j)
@@ -782,7 +800,11 @@ struct BlockArgs {
   const double *contrib_in;
   double *seg_partial;
   IterState *state;
+  const uint32_t *stage_src;  // SELL entries staged from this block: stage_val[q] = contrib_in[stage_src[q]]
+  double *stage_val;
+  uint64_t stage_begin, stage_end;
 };
+constexpr int kStageUnroll = 4;  // staged copies per thread and trip: every label load issued before the first gather
 __global__ void __launch_bounds__(kBlockThreads) cold_block_kernel(const BlockArgs a) {
   if (ld_volatile_int(&a.state->done)) return;
   const int lane = threadIdx.x & 31;
@@ -818,6 +840,22 @@ __global__ void __launch_bounds__(kBlockThreads) cold_block_kernel(const BlockAr
         if (k + j < ncols) acc += v[j];  // ascending source order inside the chunk
     }
     if (slot != ~0ull) a.seg_partial[slot] = acc;
+  }
+  // the SELL walk's values from this block (graph_build.cu step 10): edge-parallel, labels and stores streamed
+  const uint64_t threads = static_cast<uint64_t>(gridDim.x) * kBlockThreads;
+  for (uint64_t q0 = a.stage_begin + static_cast<uint64_t>(blockIdx.x) * kBlockThreads + threadIdx.x; q0 < a.stage_end;
+       q0 += threads * kStageUnroll) {
+    uint32_t src[kStageUnroll];
+    double v[kStageUnroll];
+#pragma unroll
+    for (int j = 0; j < kStageUnroll; ++j)
+      if (q0 + j * threads < a.stage_end) src[j] = ld_index(a.stage_src + q0 + j * threads, pol);
+#pragma unroll
+    for (int j = 0; j < kStageUnroll; ++j)
+      if (q0 + j * threads < a.stage_end) v[j] = ld_contrib(a.contrib_in + src[j], gpol);
+#pragma unroll
+    for (int j = 0; j < kStageUnroll; ++j)
+      if (q0 + j * threads < a.stage_end) st_stream_f64(a.stage_val + q0 + j * threads, v[j], pol);
   }
 }
 
@@ -1164,6 +1202,7 @@ SellArgs make_sell_args(const Graph &g, const double *vec, const GatherWindow &w
   s.window = window;
   s.state = g.state;
   s.sums = g.sell_sums;
+  s.stage_val = g.stage_val;
   return s;
 }
 
@@ -1307,7 +1346,8 @@ int launch_sell_stream(Graph &g, const SellArgs &s) {
   return MGB200_OK;
 }
 
-// The block passes over `vec`, one launch per non-empty block, in block order on the main stream
+// The block passes over `vec`, one launch per non-empty block, in block order on the main stream.  They also stage the
+// SELL walk's values from their blocks, so every gather path launches them before the SELL rows.
 int launch_block_passes(Graph &g, const double *vec, uint64_t *launches) {
   const uint64_t grid_cap = static_cast<uint64_t>(grid_for(g, reinterpret_cast<const void *>(cold_block_kernel)));
   for (size_t b = 0; b + 1 < g.block_slice_first.size(); ++b) {
@@ -1324,7 +1364,13 @@ int launch_block_passes(Graph &g, const double *vec, uint64_t *launches) {
     a.contrib_in = vec;
     a.seg_partial = g.seg_partial;
     a.state = g.state;
-    const int grid = static_cast<int>(std::min(grid_cap, ceil_div(a.slice_end - a.slice_begin, kWarpsPerBlock)));
+    a.stage_src = g.stage_src;
+    a.stage_val = g.stage_val;
+    a.stage_begin = g.stage_entries ? g.stage_first[b] : 0;
+    a.stage_end = g.stage_entries ? g.stage_first[b + 1] : 0;
+    const uint64_t want = std::max(ceil_div(a.slice_end - a.slice_begin, kWarpsPerBlock),
+                                   ceil_div(a.stage_end - a.stage_begin, kBlockThreads * kStageUnroll));
+    const int grid = static_cast<int>(std::min(grid_cap, want));
     cold_block_kernel<<<grid, kBlockThreads, 0, g.stream>>>(a);
     MGB_CUDA(cudaGetLastError());
     ++*launches;
@@ -1338,10 +1384,6 @@ int launch_block_passes(Graph &g, const double *vec, uint64_t *launches) {
 // kernel, joined back before the caller's row sums.  The tile kernel goes first: its CTAs need half an SM each and
 // would wait behind a full grid of segment CTAs.  The segment grid leaves `reserve_ctas` CTA slots to other kernels.
 int launch_heavy_partials(Graph &g, const HeavyArgs &h, uint64_t reserve_ctas, uint64_t *launches) {
-  // the block passes first, on the main stream: they write partials of their own, and next to the SELL epilogue they
-  // measured faster than between the SELL rows and its fork (DESIGN.md §4)
-  const int rc = launch_block_passes(g, h.contrib_in, launches);
-  if (rc) return rc;
   void (*const seg_fn)(HeavyArgs) = h.heavy_w != nullptr           ? heavy_segments_kernel<kPathRange, true>
                                     : h.window.path == kPathFlags  ? heavy_segments_kernel<kPathFlags>
                                     : h.window.path == kPathLookup ? heavy_segments_kernel<kPathLookup>
@@ -1408,8 +1450,8 @@ int launch_barrier(Graph &g) {
   return MGB200_OK;
 }
 
-// One iteration.  Main stream: (iteration 1: zero-row contribution refresh) -> SELL rows -> heavy partials (block
-// passes, tiles, segments; all inside the heavy_segments event class) ->
+// One iteration.  Main stream: (iteration 1: zero-row contribution refresh) -> block passes + SELL rows (the sell_rows
+// event class; without SELL rows the passes open the heavy_segments class) -> heavy partials (tiles, segments) ->
 // heavy finish -> [join] -> iteration end.  Side stream: the SELL epilogue, forked after the SELL rows:
 // it is the kernel that pushes contributions to the peer GPUs (NVLink-bound), so it overlaps with the
 // heavy-row kernels (L2-gather-bound) instead of queueing behind them.  Every kernel returns immediately
@@ -1437,7 +1479,9 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
     const SellArgs s = make_sell_args(g, contrib_in, window, false);
     cudaStream_t es = g.overlap_epilogue ? g.stream2 : g.stream;
     MGB_CUDA(tick(Graph::kClsSell, 0, g.stream));
-    const int rc = (g.tun.stream_kernel && g.sell_items > 0) ? launch_sell_stream(g, s) : launch_sell_rows(g, s);
+    int rc = launch_block_passes(g, contrib_in, &launches);  // with SELL rows: inside the sell_rows class
+    if (rc) return rc;
+    rc = (g.tun.stream_kernel && g.sell_items > 0) ? launch_sell_stream(g, s) : launch_sell_rows(g, s);
     if (rc) return rc;
     ++launches;
     MGB_CUDA(tick(Graph::kClsSell, 1, g.stream));
@@ -1473,7 +1517,9 @@ int launch_iteration(Graph &g, uint64_t it, const IterateConfig &cfg, uint64_t *
     const uint64_t reserve_ctas =
         (forked && g.part_world > 1 && g.tun.push_ctas > 0) ? static_cast<uint64_t>(g.sm_count) * 2 : 0;
     MGB_CUDA(tick(Graph::kClsHeavySeg, 0, g.stream));
-    int rc = launch_heavy_partials(g, h, reserve_ctas, &launches);
+    int rc = g.n_slices > 0 ? MGB200_OK : launch_block_passes(g, contrib_in, &launches);  // without: heavy class
+    if (rc) return rc;
+    rc = launch_heavy_partials(g, h, reserve_ctas, &launches);
     if (rc) return rc;
     MGB_CUDA(tick(Graph::kClsHeavySeg, 1, g.stream));
     MGB_CUDA(tick(Graph::kClsHeavyFin, 0, g.stream));
@@ -1522,6 +1568,7 @@ int launch_gather_phase(Graph &g, const double *vec_in, uint64_t *launch_count, 
     set_error("this graph handle carries no edge weights (or is partitioned)");
     return MGB200_ERR_INVALID_ARGUMENT;
   }
+  if (const int rc = launch_block_passes(g, vec_in, &launches)) return rc;  // they stage the SELL walk's values
   if (g.n_slices > 0) {
     const int rc = launch_sell_rows(g, make_sell_args(g, vec_in, window, weighted));
     if (rc) return rc;

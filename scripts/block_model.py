@@ -4,10 +4,12 @@ in how many non-empty blocks, and how long the chunks are.  With --sell-blocks 1
 putting the SELL rows into the class would move (measured slower and not built, DESIGN.md §4): their in-edges from a
 source label >= --block-from that lies in a block the heavy rows launch, one chunk per (row, block) run, and the
 SELL-32 padding of the layout with every column (`sell_pad_full`) and with the hot columns only (`sell_pad`).
+It also counts the SELL entries the build stages (graph_build.cu step 10): the SELL rows' in-edges from a launched
+block, in total (`stage_entries`) and per launched block in block order (`stage_entries_per_block`).
 
 It relabels like the build (in-degree descending, out-degree descending, id ascending), so its counts equal the
-`block_edges`, `block_chunks` and `blocks` of PageRankGraph.info for the same edges and knobs
-(tests/test_gpu_block_gather.py).
+`block_edges`, `block_chunks`, `blocks` and `stage_entries` of PageRankGraph.info for the same edges and knobs
+(tests/test_gpu_block_gather.py, tests/test_gpu_sell_stage.py).
 
     python scripts/block_model.py --scale 22 [--block-from 2097152 --block-labels 2097152 --block-chunk 16 --heavy-min 1024]
 """
@@ -31,7 +33,8 @@ def block_model(n, frm, to, block_from=2 << 20, block_labels=2 << 20, block_chun
     n_heavy = int(np.count_nonzero(indeg >= heavy_min))
     src, dst = label[frm], label[to]
     out = {"n": n, "m": len(frm), "heavy_rows": n_heavy, "heavy_edges": int(np.count_nonzero(dst < n_heavy)),
-           "block_edges": 0, "block_chunks": 0, "blocks": 0, "chunk_length_histogram": {}}
+           "block_edges": 0, "block_chunks": 0, "blocks": 0, "chunk_length_histogram": {},
+           "stage_entries": 0, "stage_entries_per_block": []}
     sell = sell_counts(n, indeg, src, dst, n_heavy, heavy_min, None, block_from, 1) if sell_blocks else None
     if block_labels == 0 or n <= block_from:
         if sell:
@@ -50,9 +53,20 @@ def block_model(n, frm, to, block_from=2 << 20, block_labels=2 << 20, block_chun
     out["chunk_length_histogram"] = {f"[{lo},{hi})" if hi < 1 << 62 else f">={lo}": int(h)
                                      for lo, hi, h in zip(edges[:-1], edges[1:], hist)}
     out["edges_per_chunk"] = out["block_edges"] / max(out["block_chunks"], 1)
+    out.update(stage_counts(indeg, src, dst, n_heavy, heavy_min, np.unique(pair % nb), block_from, labels))
     if sell_blocks:
         out.update(sell_counts(n, indeg, src, dst, n_heavy, heavy_min, np.unique(pair % nb), block_from, labels))
     return out
+
+
+def stage_counts(indeg, src, dst, n_heavy, heavy_min, launched, block_from, labels):
+    """SELL entries staged by the passes of the launched blocks (`launched`: block numbers, ascending)."""
+    sell_rows = int(np.count_nonzero((indeg >= 1) & (indeg < heavy_min)))
+    in_sell = (dst >= n_heavy) & (dst < n_heavy + sell_rows)
+    blk = np.where(src >= block_from, (src - block_from) // labels, -1)
+    staged = in_sell & np.isin(blk, launched)
+    per_block = [int(np.count_nonzero(staged & (blk == b))) for b in launched]
+    return {"stage_entries": int(staged.sum()), "stage_entries_per_block": per_block}
 
 
 def sell_counts(n, indeg, src, dst, n_heavy, heavy_min, launched, block_from, labels):

@@ -25,6 +25,8 @@ VARIANTS = {
     # unroll at 768 threads (MGB_SELL_UNROLL also sets the plain kernel's)
     "t1024": ["-DMGB_TABLE_THREADS=1024"], "t768": ["-DMGB_TABLE_THREADS=768"],
     "t768_u6": ["-DMGB_TABLE_THREADS=768", "-DMGB_SELL_UNROLL=6"], "t768_u12": ["-DMGB_TABLE_THREADS=768", "-DMGB_SELL_UNROLL=12"],
+    # the SELL walk's reads of staged values without L1 allocation (default: they may allocate)
+    "stage_noalloc": ["-DMGB_STAGE_L1=0"],
 }
 
 
