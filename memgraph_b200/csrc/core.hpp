@@ -162,7 +162,7 @@ struct Graph {
   uint64_t local_rows = 0;
   uint64_t local_edges = 0;
   uint64_t n_heavy = 0, n_sell = 0, n_zero = 0;
-  uint32_t heavy_min_degree = 0, segment_edges = 0;
+  uint32_t segment_edges = 0;  // edges per cold heavy segment (Tunables::segment_edges, or sized by the build)
   uint64_t part_start[kMaxPeers] = {};  // first global label of every partition
   uint64_t zero_lo[kMaxPeers] = {}, zero_hi[kMaxPeers] = {};  // global label range of every partition's zero rows
   bool any_zero_rows = false;
@@ -207,11 +207,11 @@ struct Graph {
   uint64_t *tile_work_begin = nullptr;  // [tile_work + 1]
   WorkQueue *tile_queue = nullptr;      // ticket of the runs (zero between launches)
   int tile_attr_bytes = 0;              // dynamic shared memory already granted to heavy_tiles_kernel
-  // block class (one partition, unweighted; graph_build.cu steps 6b and 9).  A heavy row's in-edges from labels >=
-  // block_from are summed one label block of block_labels labels at a time, so the block's part of contrib stays in L2
-  // for its whole pass.  A block chunk is <= block_chunk consecutive edges of one heavy row whose sources lie in one
-  // block; per block the chunks are sorted by length and stored as SELL-32 slices of 32-bit labels (padding = label
-  // n -> 0.0), one partial slot per lane.  A heavy row's partials: tile chunks, CSC segments, then block chunks in
+  // block class (one partition, unweighted; graph_build.cu block_edges, block_slices).  A heavy row's in-edges from
+  // labels >= block_from are summed one label block of block_labels labels at a time, so the block's part of contrib
+  // stays in L2 for its whole pass.  A block chunk is <= block_chunk consecutive edges of one heavy row whose sources
+  // lie in one block; per block the chunks are sorted by length and stored as SELL-32 slices of 32-bit labels (padding =
+  // label n -> 0.0), one partial slot per lane.  A heavy row's partials: tile chunks, CSC segments, then block chunks in
   // block order.
   uint64_t block_edges = 0, block_chunks = 0;
   uint64_t block_labels = 0;                // labels per block (MGB200_BLOCK_LABELS, raised to keep <= kMaxBlocks)
@@ -221,9 +221,9 @@ struct Graph {
   uint64_t *bslice_colbase = nullptr;       // [block_slices + 1] in units of 32-entry columns
   uint32_t *block_idx = nullptr;            // [32 * columns] source labels, pad = n
   uint64_t *block_slot = nullptr;           // [32 * block_slices] partial written by each lane; ~0 = padding lane
-  // SELL staging (graph_build.cu step 10): a SELL entry whose source lies in a launched block is read by the walk from
-  // stage_val, which that block's pass fills (stage_val[q] = vec[stage_src[q]]) while the block sits in L2.  Slots are
-  // ordered by (block, position in sell_idx), so a column's lanes read neighbouring slots.
+  // SELL staging (graph_build.cu sell_staging): a SELL entry whose source lies in a launched block is read by the walk
+  // from stage_val, which that block's pass fills (stage_val[q] = vec[stage_src[q]]) while the block sits in L2.  Slots
+  // are ordered by (block, position in sell_idx), so a column's lanes read neighbouring slots.
   uint64_t stage_entries = 0;
   std::vector<uint64_t> stage_first;  // host: [launched blocks + 1] first slot of every block's pass
   uint32_t *stage_src = nullptr;      // [stage_entries] source label of every slot
@@ -264,6 +264,7 @@ struct Graph {
   bool poisoned = false;  // a peer barrier timed out: the partitions' barrier counters may disagree; runs are refused
 
   uint64_t resident_bytes = 0;
+  std::vector<void *> device_arrays;  // every device array the build kept (keep_alloc): free_graph frees them
   uint64_t build_peak_bytes = 0;  // highest device memory in use seen during the build (transients included)
   double build_ms = 0.0;
   double upload_ms = 0.0;  // host COO -> device (mgb200_graph_create_host*), wall clock
@@ -282,7 +283,7 @@ struct Graph {
   mutable const void *occ_kernel[kOccSlots] = {};
   mutable int occ_blocks[kOccSlots] = {};
   mutable int occ_cached = 0;
-  struct Tunables {  // environment, read once per graph in build_graph()
+  struct Tunables {  // environment, read once per graph (graph_build.cu read_tunables)
     uint64_t l2_hot_mb = 16;     // MGB200_L2_HOT_MB: evict-last window of the gathered vector.  H100 SXM (50 MB L2, 700 W),
                                  // RMAT scale-26: 16 MB beat 8 / 24 / 32 / 48 / 64 (10.1 vs 10.2-10.8 ms per iteration)
     long l1_hot_k = 16;          // MGB200_L1_HOT_K: hottest labels (x1024) allowed to allocate in L1; <0 = no L1 hints
@@ -307,8 +308,14 @@ struct Graph {
     uint32_t block_chunk = 16;         // MGB200_BLOCK_CHUNK: most edges of one block chunk (DESIGN.md §4: a pass lasts
                                        // as long as its longest chunk's chain of dependent gathers)
     int sell_stage = -1;               // MGB200_SELL_STAGE: 1 stage, 0 never, -1 (default) when the gathered vector is
-                                       // larger than the device's L2 (graph_build.cu step 10)
+                                       // larger than the device's L2 (graph_build.cu sell_staging)
     unsigned long long barrier_timeout_ms = 20000;  // MGB200_BARRIER_TIMEOUT_MS
+    uint32_t heavy_min_degree = 1024;  // MGB200_HEAVY_MIN_DEGREE: in-degree from which a row is heavy
+    uint32_t segment_edges = 0;        // MGB200_SEGMENT_EDGES: edges per cold heavy segment; unset (0): sized by the build
+    uint32_t tile_runs = 0;            // MGB200_TILE_RUNS: runs of heavy_tiles_kernel (default 8 per SM)
+    uint32_t sell_items = 0;           // MGB200_SELL_ITEMS: work items of the streaming SELL kernel (default 32 per SM)
+    uint32_t slice_cost = 8;           // MGB200_SLICE_COST: columns a slice start costs in sell_rows_kernel's work items
+    uint32_t sell_work_items = 0;      // MGB200_SELL_WORK_ITEMS: work items of sell_rows_kernel (0: by slices per warp)
   } tun;
   // hot thresholds in LOCAL label units (label - first label of the owning partition); one definition for the
   // build-time index flags and the run-time gather window

@@ -117,7 +117,7 @@ __device__ __forceinline__ GatherPolicy make_gather_policy(const double *contrib
 // and the degree-sorted labelling makes "hottest" a prefix -- 21 % of all gathers of RMAT-26 go to the first 16 K
 // labels, 27 % to the first 28 K (scripts/topk_share.py).  One partition: slot = label (label < table_n).  Several
 // partitions: the build stored the slot in the index itself, code 01 in bits 31/30 (graph_build.cu IndexFlags).
-// kStaged (the SELL walk on the range path): an index with kIdxStaged set is a slot of `staged` (graph_build.cu step 10),
+// kStaged (the SELL walk on the range path): an index with kIdxStaged set is a slot of `staged` (graph_build.cu sell_staging),
 // filled by the block pass of its source's block; it is read once per gather, evict-first in L2.
 #ifndef MGB_STAGE_L1
 #define MGB_STAGE_L1 1  // staged reads: 1 default L1 allocation (neighbouring columns share sectors), 0 no_allocate
@@ -785,7 +785,7 @@ __global__ void __launch_bounds__(kTileThreads, 2) heavy_tiles_kernel(const Tile
   }
 }
 
-// Block passes (graph_build.cu step 9): the heavy rows' in-edges from labels >= block_from, one label block per launch,
+// Block passes (graph_build.cu block_slices): the heavy rows' in-edges from labels >= block_from, one label block per launch,
 // so the block's part of contrib is read from HBM about once per pass instead of costing a sector per gather.  One warp
 // per slice, one lane per chunk: the lane adds its chunk in ascending source order and stores the chunk's partial (no
 // atomics, the same bits every run).
@@ -841,7 +841,7 @@ __global__ void __launch_bounds__(kBlockThreads) cold_block_kernel(const BlockAr
     }
     if (slot != ~0ull) a.seg_partial[slot] = acc;
   }
-  // the SELL walk's values from this block (graph_build.cu step 10): edge-parallel, labels and stores streamed
+  // the SELL walk's values from this block (graph_build.cu sell_staging): edge-parallel, labels and stores streamed
   const uint64_t threads = static_cast<uint64_t>(gridDim.x) * kBlockThreads;
   for (uint64_t q0 = a.stage_begin + static_cast<uint64_t>(blockIdx.x) * kBlockThreads + threadIdx.x; q0 < a.stage_end;
        q0 += threads * kStageUnroll) {

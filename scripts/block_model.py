@@ -1,11 +1,11 @@
-"""Counting model of the block class (graph_build.cu steps 6b and 9, one partition): which in-edges of the heavy rows
-come from a source label >= --block-from, how many (row, label block) chunks of at most --block-chunk edges they make,
-in how many non-empty blocks, and how long the chunks are.  With --sell-blocks 1 (the default) it also counts what
-putting the SELL rows into the class would move (measured slower and not built, DESIGN.md §4): their in-edges from a
-source label >= --block-from that lies in a block the heavy rows launch, one chunk per (row, block) run, and the
-SELL-32 padding of the layout with every column (`sell_pad_full`) and with the hot columns only (`sell_pad`).
-It also counts the SELL entries the build stages (graph_build.cu step 10): the SELL rows' in-edges from a launched
-block, in total (`stage_entries`) and per launched block in block order (`stage_entries_per_block`).
+"""Counting model of the block class (graph_build.cu block_edges and block_slices, one partition): which in-edges of the
+heavy rows come from a source label >= --block-from, how many (row, label block) chunks of at most --block-chunk edges
+they make, in how many non-empty blocks, and how long the chunks are.  With --sell-blocks 1 (the default) it also counts
+what putting the SELL rows into the class would move (measured slower and not built, DESIGN.md §4): their in-edges from
+a source label >= --block-from that lies in a block the heavy rows launch, one chunk per (row, block) run, and the
+SELL-32 padding of the layout with every column (`sell_pad_full`) and with the hot columns only (`sell_pad`). It also
+counts the SELL entries the build stages (graph_build.cu sell_staging): the SELL rows' in-edges from a launched block,
+in total (`stage_entries`) and per launched block in block order (`stage_entries_per_block`).
 
 It relabels like the build (in-degree descending, out-degree descending, id ascending), so its counts equal the
 `block_edges`, `block_chunks`, `blocks` and `stage_entries` of PageRankGraph.info for the same edges and knobs

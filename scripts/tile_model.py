@@ -1,5 +1,6 @@
-"""Counting model of the heavy rows' tile class (graph_build.cu step 7, one partition): how many in-edges of the heavy
-rows come from a source in the tiled prefix, how many (row, tile) chunks they make, and how long the chunks are.
+"""Counting model of the heavy rows' tile class (graph_build.cu heavy_class and tile_slices, one partition): how many
+in-edges of the heavy rows come from a source in the tiled prefix, how many (row, tile) chunks they make, and how long
+the chunks are.
 
 It relabels like the build (in-degree descending, out-degree descending, id ascending), so its counts equal the
 `tiled_edges` / `tile_chunks` of PageRankGraph.info for the same edges and knobs (tests/test_gpu_tiles.py).

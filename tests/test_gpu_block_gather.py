@@ -1,7 +1,7 @@
-"""-m gpu: the block class (graph_build.cu steps 6b and 9, pagerank_kernels.cu cold_block_kernel).  The heavy rows'
-in-edges from labels >= MGB200_BLOCK_FROM are summed one label block at a time into partials of their own.  Only the
-order of the FP64 additions inside a heavy row may change: every layout the knobs allow must match the oracle, repeat bit
-for bit, agree with the class turned off, and count what scripts/block_model.py counts."""
+"""-m gpu: the block class (graph_build.cu block_edges and block_slices, pagerank_kernels.cu cold_block_kernel).  The
+heavy rows' in-edges from labels >= MGB200_BLOCK_FROM are summed one label block at a time into partials of their
+own.  Only the order of the FP64 additions inside a heavy row may change: every layout the knobs allow must match the
+oracle, repeat bit for bit, agree with the class turned off, and count what scripts/block_model.py counts."""
 import os
 import sys
 

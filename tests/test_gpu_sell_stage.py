@@ -1,4 +1,4 @@
-"""-m gpu: SELL staging (graph_build.cu step 10, pagerank_kernels.cu cold_block_kernel / sell_walk).  A SELL entry whose
+"""-m gpu: SELL staging (graph_build.cu sell_staging, pagerank_kernels.cu cold_block_kernel / sell_walk).  A SELL entry whose
 source lies in a block that has a pass is read from a value that pass staged, not from the gathered vector.  The
 value is the same double and the add order inside a row is unchanged, so every algorithm that shares the gather must
 give the same bits with staging on and off, count what scripts/block_model.py counts, and stage nothing where the

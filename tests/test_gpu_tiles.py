@@ -1,4 +1,4 @@
-"""-m gpu: the heavy rows' tile class (graph_build.cu step 7c, pagerank_kernels.cu heavy_tiles_kernel).  A heavy row's
+"""-m gpu: the heavy rows' tile class (graph_build.cu tile_slices, pagerank_kernels.cu heavy_tiles_kernel).  A heavy row's
 in-edges from the tiled hot prefix are summed per (row, tile) chunk from a shared-memory copy of that tile, the rest by
 edge segments.  Only the order of the FP64 additions inside a heavy row may change: every layout the knobs allow must
 match the oracle, repeat bit for bit, and count what scripts/tile_model.py counts."""
