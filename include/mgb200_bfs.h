@@ -202,6 +202,37 @@ int mgb200_weighted_shortest_paths(uint64_t n, uint64_t m, const uint64_t *from,
                                    const double *weight, uint64_t source, int direction, int64_t upper_bound,
                                    double *dist_out, int32_t *hops_out);
 
+/*
+ * Maximum bipartite matching of the undirected multigraph view on the same device graph: the answer of the reference's
+ * bipartite_matching.max (mage/cpp/bipartite_matching_module).  A breadth-first forest from each component's smallest
+ * id colours the graph; a self-loop or an edge between two vertices of the same forest level (an odd cycle) means the
+ * graph is not bipartite and the answer is 0.  Otherwise the even-depth vertices are the left side, and greedy rounds
+ * followed by alternating breadth-first searches from every free left vertex (one phase per search, paths flipped in
+ * parallel) grow the matching until a search finds no augmenting path.  Every choice is a minimum over vertex ids, so
+ * two runs give byte-identical outputs and stats (run_ms aside).  Without a device every call fails with
+ * MGB200_ERR_CUDA.
+ */
+typedef struct mgb200_matching_stats {
+  int bipartite;              /* 0: a self-loop or an odd cycle; nothing matched                  */
+  uint64_t left_vertices;     /* even forest depth: the side the searches start from (0 if not bipartite) */
+  uint64_t matched;           /* pairs = the reference procedure's answer                          */
+  uint64_t initial_matched;   /* pairs after the greedy rounds                                     */
+  uint64_t phases;            /* alternating searches, the last one fruitless                      */
+  uint32_t max_levels;        /* deepest search level of any phase                                 */
+  uint64_t edges_inspected;   /* adjacency entries read: colouring, greedy and searches together   */
+  double run_ms;              /* CUDA-event time, first kernel .. last output (no transfers)        */
+  uint64_t kernel_launches;
+} mgb200_matching_stats;
+
+/* mate_out: n int64 (partner id or -1); cover_out: n uint8 (a minimum vertex cover by Konig's theorem: 1 for its
+ * vertices, as many as there are pairs); host memory, either may be NULL.  Not bipartite: mate all -1, cover all 0.
+ * should_abort (may be NULL) is polled between phases; non-zero -> MGB200_ERR_ABORTED.  stats may be NULL. */
+int mgb200_bipartite_matching_run(mgb200_bfs_graph *g, int (*should_abort)(void *user), void *abort_user,
+                                  int64_t *mate_out, uint8_t *cover_out, mgb200_matching_stats *stats);
+/* One shot on device 0: host COO (uint64 endpoints < n) -> the reference's answer. */
+int mgb200_maximum_bipartite_matching(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to,
+                                      uint64_t *matched_out);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -55,6 +55,11 @@ class WspStats(ctypes.Structure):
                 ("kernel_launches", u64)]
 
 
+class MatchingStats(ctypes.Structure):
+    _fields_ = [("bipartite", i32), ("left_vertices", u64), ("matched", u64), ("initial_matched", u64), ("phases", u64),
+                ("max_levels", u32), ("edges_inspected", u64), ("run_ms", f64), ("kernel_launches", u64)]
+
+
 class KatzStats(ctypes.Structure):
     _fields_ = [("iterations", u64), ("max_out_degree", u64), ("gamma", f64), ("iterate_ms", f64),
                 ("kernel_launches", u64), ("tie_order_runs", u64)]
@@ -126,6 +131,8 @@ EXPORTS = {
     "mgb200_bfs_graph_set_weights": (i32, [vp, u64, vp, vp, vp]),
     "mgb200_wsp_run": (i32, [vp, u64, i32, ctypes.c_int64, ABORT_FN, vp, vp, vp, ctypes.POINTER(WspStats)]),
     "mgb200_weighted_shortest_paths": (i32, [u64, u64, vp, vp, vp, u64, i32, ctypes.c_int64, vp, vp]),
+    "mgb200_bipartite_matching_run": (i32, [vp, ABORT_FN, vp, vp, vp, ctypes.POINTER(MatchingStats)]),
+    "mgb200_maximum_bipartite_matching": (i32, [u64, u64, vp, vp, ctypes.POINTER(u64)]),
     # include/mgb200_katz.h
     "mgb200_katz_run": (i32, [vp, f64, f64, u64, vp, ctypes.POINTER(KatzStats)]),
     "mgb200_katz_centrality": (i32, [u64, u64, vp, vp, f64, f64, u64, vp, ctypes.POINTER(u64)]),

@@ -5,8 +5,8 @@
     memgraph_b200/_build/libmgp_fake_host.so     fake mgp host used by the tests to load query modules without Memgraph
     memgraph_b200/_build/<module>.so             the other query modules (gpu_bfs, katz_centrality, betweenness_centrality,
                                                  weakly_connected_components, bridges, biconnected_components,
-                                                 gpu_wsp, cugraph.* including cugraph.hits), same linking
-                                                 as pagerank.so
+                                                 gpu_wsp, bipartite_matching, cugraph.* including cugraph.hits),
+                                                 same linking as pagerank.so
 
 Objects are rebuilt only when a source or header is newer.  `python -m memgraph_b200.build` builds everything.
 """
@@ -33,9 +33,9 @@ NVCC_FLAGS = [
     "-diag-suppress", "1444",  # cub::TransformInputIterator deprecation notice
 ]
 CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu",
-                "wcc.cu", "biconnectivity.cu", "wsp.cu", "hits.cu"]
+                "wcc.cu", "biconnectivity.cu", "wsp.cu", "hits.cu", "bipartite_matching.cu"]
 HEADERS = [os.path.join(CSRC, "core.hpp"), os.path.join(CSRC, "bfs_graph.hpp"), os.path.join(CSRC, "rmat.hpp"), os.path.join(CSRC, "sell_stream.cuh"),
-           os.path.join(CSRC, "union_find.cuh"),
+           os.path.join(CSRC, "union_find.cuh"), os.path.join(CSRC, "undirected_walk.cuh"),
            os.path.join(INCLUDE, "mgb200_pagerank.h"), os.path.join(INCLUDE, "mgb200_bfs.h"),
            os.path.join(INCLUDE, "mgb200_katz.h"), os.path.join(INCLUDE, "mgb200_personalized.h"), os.path.join(CSRC, "katz_heap.hpp"),
            os.path.join(INCLUDE, "mgp_abi.h"), os.path.join(CSRC, "mgp_module_common.hpp")]
@@ -94,6 +94,7 @@ MODULES = {
     "biconnectivity_modules.cpp": [("bridges.so", ["-DMGB200_BRIDGES=1"], "bridges_module"),
                                    ("biconnected_components.so", ["-DMGB200_BRIDGES=0"], "biconnected_components_module")],
     "gpu_wsp_module.cpp": [("gpu_wsp.so", [], "wsp_module")],
+    "bipartite_matching_module.cpp": [("bipartite_matching.so", [], "bipartite_matching_module")],
 }
 
 # The fake mgp hosts the tests load modules through (test infrastructure, so they live with the tests): library ->

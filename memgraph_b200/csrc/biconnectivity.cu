@@ -4,9 +4,8 @@
 // mage/cpp/biconnected_components_module; restated in oracle/biconnectivity_oracle.c), which run a recursive
 // Hopcroft-Tarjan DFS on one host thread.  Here both come from one spanning forest (Tarjan-Vishkin), integer work only:
 //   roots     the union-find of wcc.cu over the COO: every component's root is its smallest id
-//   forest    a level-synchronous BFS over the undirected view (out-list, then in-list) from all roots at once; the
-//             parent of a vertex is its smallest-id neighbour in the previous level (atomicMin), so the forest does not
-//             depend on thread order.  Every level's vertices are kept (order[] + level offsets on the host)
+//   forest    undirected_walk.cuh's level-synchronous BFS over the undirected view (out-list, then in-list) from all
+//             roots at once; the parent of a vertex is its smallest-id neighbour in the previous level
 //   size      levels bottom-up, atomicAdd of each subtree size into the parent
 //   pre       the non-roots sorted by (parent, id) once (stable cub radix sort on the parent); a vertex's sibling offset
 //             is the exclusive sum of its earlier siblings' sizes; levels top-down, pre(v) = pre(parent) + 1 + offset.
@@ -20,10 +19,10 @@
 //             root, with low(v) < pre(p) or high(v) >= pre(p) + size(p)
 //   per edge  x = the endpoint with the larger pre; bridge = bridge(x) && parent(x) is the other end; block = e(x).
 //             Blocks are numbered in the order of their first edge in the COO (an exclusive scan of first-edge flags)
-// The entry scans run a thread per vertex up to kThreadEntries entries, a warp up to kWarpEntries and a block above.
+// The entry scans are undirected_walk.cuh's: a thread per vertex up to kThreadEntries entries, a warp up to
+// kWarpEntries and a block above.
 // The forest costs one host round trip per BFS level, and every sweep one launch per level: deep forests (long paths)
 // are launch-bound, see DESIGN.md section 9.
-#include <cooperative_groups.h>
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -35,32 +34,11 @@
 #include "bfs_graph.hpp"
 #include "core.hpp"
 #include "mgb200_bfs.h"
+#include "undirected_walk.cuh"
 #include "union_find.cuh"
-
-namespace cg = cooperative_groups;
 
 namespace mgb200 {
 namespace {
-
-constexpr uint32_t kNone = 0xffffffffu;
-constexpr uint64_t kThreadEntries = 16;  // entries a single thread walks
-constexpr uint64_t kWarpEntries = 4096;  // above this, a block per vertex
-
-struct Lists {  // the undirected view: out-list, then in-list
-  const uint64_t *out_ptr;
-  const uint32_t *out_adj;
-  const uint64_t *in_ptr;
-  const uint32_t *in_adj;
-  __device__ __forceinline__ uint64_t degree(uint32_t u) const {
-    return out_ptr[u + 1] - out_ptr[u] + in_ptr[u + 1] - in_ptr[u];
-  }
-};
-
-struct Split {  // one entry-scan pass: vertices queued for a warp (front of the work list) or a block (back)
-  unsigned int mid;
-  unsigned int heavy;
-  unsigned long long next;  // BFS: vertices appended to the next level
-};
 
 struct Counters {
   Split split[2];  // BFS level L uses split[L & 1]; its thread kernel clears the other for level L + 1
@@ -70,42 +48,11 @@ struct Counters {
   unsigned long long trees;
 };
 
-// Appends w to dst at a slot reserved with one atomic per group of converged threads.
-__device__ __forceinline__ void append(uint32_t w, uint32_t *dst, unsigned long long *counter) {
-  cg::coalesced_group active = cg::coalesced_threads();
-  unsigned long long base = 0;
-  if (active.thread_rank() == 0) base = atomicAdd(counter, static_cast<unsigned long long>(active.size()));
-  base = active.shfl(base, 0);
-  dst[base + active.thread_rank()] = w;
-}
-
 __device__ __forceinline__ bool is_ancestor(uint32_t a, uint32_t b, const uint32_t *pre, const uint32_t *size) {
   return pre[a] <= pre[b] && pre[b] < pre[a] + size[a];
 }
 
 // ---- entry scans: an op walks the entries [rank, degree) of u with stride `width` ---------------------------------
-
-struct BfsOp {  // discovers the next level; the parent is the smallest frontier neighbour
-  Lists g;
-  int32_t *depth;
-  uint32_t *tree_parent;
-  uint32_t *next;  // order + end of the current level
-  unsigned long long *next_count;
-  int32_t next_depth;
-  __device__ __forceinline__ void operator()(uint32_t u, uint64_t rank, uint64_t width) const {
-    const uint64_t ob = g.out_ptr[u], od = g.out_ptr[u + 1] - ob;
-    const uint64_t ib = g.in_ptr[u], id = g.in_ptr[u + 1] - ib;
-    for (uint64_t i = rank; i < od + id; i += width) {
-      const uint32_t w = i < od ? g.out_adj[ob + i] : g.in_adj[ib + (i - od)];
-      int32_t d = *(reinterpret_cast<volatile int32_t *>(depth) + w);
-      if (d == -1) {
-        if (atomicCAS(depth + w, -1, next_depth) == -1) append(w, next, next_count);
-        d = next_depth;  // whoever won set this level
-      }
-      if (d == next_depth) atomicMin(tree_parent + w, u);
-    }
-  }
-};
 
 struct LocalOp {  // min / max of pre over the entries, one occurrence of the tree parent left out
   Lists g;
@@ -145,80 +92,12 @@ struct LocalOp {  // min / max of pre over the entries, one occurrence of the tr
   }
 };
 
-// Items [lo, hi) of `items` (or the ids themselves when items is null): short lists walked by one thread, the others
-// queued for walk_warp_kernel / walk_block_kernel.  Block 0 also clears `clear` for the next pass.
-template <class Op>
-__global__ void __launch_bounds__(kThreads) walk_thread_kernel(uint64_t lo, uint64_t hi, const uint32_t *items,
-                                                               uint64_t n, Op op, uint32_t *work, Split *split,
-                                                               Split *clear, unsigned long long *inspected) {
-  if (clear && first_thread() == 0) *clear = Split{0, 0, 0};
-  unsigned long long walked = 0;
-  for (uint64_t i = lo + first_thread(); i < lo + warp_rounded(hi - lo); i += thread_count()) {
-    if (i >= hi) continue;
-    const uint32_t u = items ? items[i] : static_cast<uint32_t>(i);
-    const uint64_t deg = op.g.degree(u);
-    if (deg <= kThreadEntries) {
-      op(u, 0, 1);
-      walked += deg;
-    } else if (deg <= kWarpEntries) {
-      work[atomicAdd(&split->mid, 1u)] = u;
-    } else {
-      work[n - 1 - atomicAdd(&split->heavy, 1u)] = u;
-    }
-  }
-  add_warp_sum(walked, inspected);
-}
-
-template <class Op>
-__global__ void __launch_bounds__(kThreads) walk_warp_kernel(Op op, const uint32_t *work, const Split *split,
-                                                             unsigned long long *inspected) {
-  const uint32_t count = split->mid;
-  const uint32_t lane = threadIdx.x & 31;
-  unsigned long long walked = 0;
-  for (uint64_t w = first_thread() >> 5; w < count; w += thread_count() >> 5) {
-    const uint32_t u = work[w];
-    op(u, lane, 32);
-    if (lane == 0) walked += op.g.degree(u);
-  }
-  if (lane == 0 && walked) atomicAdd(inspected, walked);
-}
-
-template <class Op>
-__global__ void __launch_bounds__(kThreads) walk_block_kernel(uint64_t n, Op op, const uint32_t *work,
-                                                              const Split *split, unsigned long long *inspected) {
-  const uint32_t count = split->heavy;
-  unsigned long long walked = 0;
-  for (uint32_t b = blockIdx.x; b < count; b += gridDim.x) {
-    const uint32_t u = work[n - 1 - b];
-    op(u, threadIdx.x, blockDim.x);
-    if (threadIdx.x == 0) walked += op.g.degree(u);
-  }
-  if (threadIdx.x == 0 && walked) atomicAdd(inspected, walked);
-}
-
 // ---- per-vertex and per-edge passes ---------------------------------------------------------------------------------
-
-__global__ void __launch_bounds__(kThreads) iota_kernel(uint64_t n, uint32_t *a) {
-  for (uint64_t v = first_thread(); v < n; v += thread_count()) a[v] = static_cast<uint32_t>(v);
-}
 
 __global__ void __launch_bounds__(kThreads) link_edges_kernel(uint64_t m, const uint32_t *from, const uint32_t *to,
                                                               uint32_t *parent) {
   for (uint64_t e = first_thread(); e < m; e += thread_count())
     if (from[e] != to[e]) link(from[e], to[e], parent);
-}
-
-// Roots start level 0; every other vertex is undiscovered, its parent kNone until a frontier neighbour claims it.
-__global__ void __launch_bounds__(kThreads) forest_init_kernel(uint64_t n, const uint32_t *uf, int32_t *depth,
-                                                               uint32_t *tree_parent, uint32_t *size, uint32_t *order,
-                                                               Counters *counters) {
-  for (uint64_t v = first_thread(); v < n; v += thread_count()) {
-    const bool root = uf[v] == v;
-    depth[v] = root ? 0 : -1;
-    tree_parent[v] = kNone;
-    size[v] = 1;
-    if (root) append(static_cast<uint32_t>(v), order, &counters->split[1].next);  // level 0 clears it after the read
-  }
 }
 
 __global__ void __launch_bounds__(kThreads) size_level_kernel(uint64_t lo, uint64_t hi, const uint32_t *order,
@@ -370,20 +249,6 @@ __global__ void __launch_bounds__(kThreads) number_kernel(uint64_t m, const uint
   add_warp_sum(firsts, &counters->components);
 }
 
-// One entry-scan pass over items [lo, hi): thread, warp and block kernels.
-template <class Op>
-void walk(const mgb200_bfs_graph &g, uint64_t lo, uint64_t hi, const uint32_t *items, const Op &op, uint32_t *work,
-          Split *split, Split *clear, Counters *counters, uint64_t *launches) {
-  const uint64_t count = hi - lo;
-  walk_thread_kernel<Op><<<blocks_for(count, g.sm_count, 8), kThreads, 0, g.stream>>>(
-      lo, hi, items, g.n, op, work, split, clear, &counters->inspected);
-  walk_warp_kernel<Op><<<blocks_for(count * 32, g.sm_count, 16), kThreads, 0, g.stream>>>(op, work, split,
-                                                                                           &counters->inspected);
-  walk_block_kernel<Op><<<static_cast<int>(std::min<uint64_t>(count, static_cast<uint64_t>(g.sm_count) * 8)), kThreads,
-                          0, g.stream>>>(g.n, op, work, split, &counters->inspected);
-  *launches += 3;
-}
-
 }  // namespace
 }  // namespace mgb200
 
@@ -415,7 +280,6 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
   MGB_CUDA(cudaSetDevice(g->device));
   cudaStream_t st = g->stream;
   const Lists lists{g->out_ptr, g->out_adj, g->in_ptr, g->in_adj};
-  int32_t *depth = g->depth;
   uint32_t *order = g->queue[0], *work = g->queue[1];
 
   DeviceBuffers buf;
@@ -468,7 +332,6 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
 
   const int grid_n = blocks_for(n, g->sm_count, 8), grid_m = blocks_for(m, g->sm_count, 8);
   uint64_t launches = 0;
-  unsigned long long *host_next = g->host_counters;  // pinned
   MGB_CUDA(cudaEventRecord(g->ev0, st));
   MGB_CUDA(cudaMemsetAsync(counters, 0, sizeof(Counters), st));
   MGB_CUDA(cudaMemsetAsync(first_edge, 0xff, n * sizeof(unsigned long long), st));
@@ -477,26 +340,13 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
   iota_kernel<<<grid_n, kThreads, 0, st>>>(n, uf);
   if (m) link_edges_kernel<<<grid_m, kThreads, 0, st>>>(m, d_from, d_to, uf);
   compress_kernel<<<grid_n, kThreads, 0, st>>>(n, uf);
-  forest_init_kernel<<<grid_n, kThreads, 0, st>>>(n, uf, depth, tree_parent, size, order, counters);
-  launches += m ? 4 : 3;
+  launches += m ? 3 : 2;
 
   // forest: one BFS level per round trip; level L's vertices are order[level[L], level[L + 1])
-  std::vector<uint64_t> level{0};
-  MGB_CUDA(cudaMemcpyAsync(host_next, &counters->split[1].next, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  MGB_CUDA(cudaStreamSynchronize(st));
-  level.push_back(*host_next);
-  for (uint32_t L = 0;; ++L) {
-    const uint64_t lo = level[L], hi = level[L + 1];
-    if (lo == hi) break;
-    // level L uses split[L & 1] and clears the other set, whose count the host has just read
-    Split *split = &counters->split[L & 1], *clear = &counters->split[(L + 1) & 1];
-    const BfsOp op{lists, depth, tree_parent, order + hi, &split->next, static_cast<int32_t>(L + 1)};
-    walk(*g, lo, hi, order, op, work, split, clear, counters, &launches);
-    MGB_CUDA(cudaMemcpyAsync(host_next, &split->next, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    MGB_CUDA(cudaStreamSynchronize(st));
-    level.push_back(hi + *host_next);
-  }
-  MGB_CUDA(cudaGetLastError());
+  std::vector<uint64_t> level;
+  const int rc = bfs_forest(*g, uf, tree_parent, size, order, work, counters->split, &counters->inspected, &level,
+                            &launches);
+  if (rc) return rc;
   const uint32_t levels = static_cast<uint32_t>(level.size() - 2);  // the last entry closes an empty level
   if (level[levels] != n) {
     set_error("biconnectivity: the forest does not span the graph (internal error)");
@@ -529,8 +379,8 @@ int mgb200_biconnectivity_run(mgb200_bfs_graph *g, uint64_t m, const uint64_t *f
   low_high_init_kernel<<<grid_n, kThreads, 0, st>>>(n, pre, low, high);
   ++launches;
   MGB_CUDA(cudaMemsetAsync(&counters->split[0], 0, sizeof(Split), st));
-  walk(*g, 0, n, nullptr, LocalOp{lists, pre, tree_parent, low, high}, work, &counters->split[0], nullptr, counters,
-       &launches);
+  walk(*g, 0, n, nullptr, LocalOp{lists, pre, tree_parent, low, high}, work, &counters->split[0], nullptr,
+       &counters->inspected, &launches);
   for (uint32_t L = levels - 1; L >= 1; --L) {
     low_high_level_kernel<<<blocks_for(level[L + 1] - level[L], g->sm_count, 8), kThreads, 0, st>>>(
         level[L], level[L + 1], order, tree_parent, low, high);

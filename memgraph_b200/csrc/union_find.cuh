@@ -1,7 +1,7 @@
-// memgraph_b200/csrc/union_find.cuh -- the lock-free union-find shared by weakly connected components (wcc.cu) and
-// biconnectivity (biconnectivity.cu): one uint32 parent per element.  A link hooks the larger of two roots under the
-// smaller one with atomicCAS and a compression only shortens paths, so parent[x] <= x always holds and every root is
-// its set's smallest element, whatever order the threads link in.
+// memgraph_b200/csrc/union_find.cuh -- the lock-free union-find shared by weakly connected components (wcc.cu),
+// biconnectivity (biconnectivity.cu) and bipartite matching (bipartite_matching.cu): one uint32 parent per element.
+// A link hooks the larger of two roots under the smaller one with atomicCAS and a compression only shortens paths, so
+// parent[x] <= x always holds and every root is its set's smallest element, whatever order the threads link in.
 #pragma once
 
 #include <cstdint>
@@ -11,6 +11,13 @@ namespace {
 
 __device__ __forceinline__ uint32_t load(const uint32_t *parent, uint32_t i) {
   return *(reinterpret_cast<const volatile uint32_t *>(parent) + i);  // other threads hook roots concurrently
+}
+
+// a[v] = v: every element its own set.
+__global__ void __launch_bounds__(256) iota_kernel(uint64_t n, uint32_t *a) {
+  for (uint64_t v = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < n;
+       v += static_cast<uint64_t>(gridDim.x) * blockDim.x)
+    a[v] = static_cast<uint32_t>(v);
 }
 
 // Union of the sets of u and v: the larger root is hooked under the smaller one.
