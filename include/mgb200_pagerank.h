@@ -142,6 +142,14 @@ int mgb200_graph_get_info(const mgb200_graph *g, mgb200_graph_info *info);
 int mgb200_pagerank_run(mgb200_graph *g, const mgb200_run_params *params, double *rank_out,
                         mgb200_run_stats *stats);
 
+/* One gather alone: y[v] = sum over the edges u -> v of x[u] (times the edge's weight when `weighted`), with the
+ * kernels, layout and summation order every PageRank-layout algorithm iterates, and no epilogue.  x and y hold
+ * node_count doubles in ORIGINAL vertex-id order, in host memory (on_device = 0) or on the graph's device (1).
+ * Single-partition handles only; weighted = 1 needs a handle built with edge weights
+ * (mgb200_graph_create_host_weighted_u32).  The call overwrites the handle's contribution buffer: a later run, Katz or
+ * cuGraph-PageRank call on the handle starts from scratch, as it does anyway. */
+int mgb200_graph_gather(mgb200_graph *g, const double *x, double *y, int on_device, int weighted);
+
 /* PageRankGraph(n, m, edges) + ParallelIterativePageRank(graph, ...) in one call, host buffers in
  * and out -- what PagerankWrapper does between ingest and record emission
  * (pagerank_module.cpp:100-102).  number_of_threads is accepted for signature fidelity: 0 is the

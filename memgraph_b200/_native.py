@@ -105,6 +105,7 @@ EXPORTS = {
     "mgb200_graph_destroy": (None, [vp]),
     "mgb200_graph_get_info": (i32, [vp, ctypes.POINTER(GraphInfo)]),
     "mgb200_pagerank_run": (i32, [vp, ctypes.POINTER(RunParams), vp, ctypes.POINTER(RunStatsC)]),
+    "mgb200_graph_gather": (i32, [vp, vp, vp, i32, i32]),
     "mgb200_parallel_iterative_pagerank": (i32, [u64, u64, vp, vp, u64, f64, f64, u32, vp, ctypes.POINTER(u64)]),
     "mgb200_parallel_iterative_pagerank_multi": (i32, [u64, u64, vp, vp, u64, f64, f64, u32, u32, vp, vp,
                                                        ctypes.POINTER(u64)]),

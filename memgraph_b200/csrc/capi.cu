@@ -278,8 +278,10 @@ int iterate(Graph &g, const mgb200_run_params &p, mgb200_run_stats &stats) {
 }  // namespace mgb200
 
 namespace mgb200 {
+// personalized.cu
 int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double *d_out_original_order,
                              mgb200_cugraph_stats *stats);
+int gather_once(Graph &g, const double *d_x, double *d_y, bool weighted);
 // hits.cu
 int hits_permutations(Graph &f, Graph &t, uint32_t *t_of_f, uint32_t *f_of_t);
 uint64_t hits_scratch_doubles(uint64_t n);
@@ -921,6 +923,31 @@ int mgb200_cugraph_pagerank_run(mgb200_graph *h, const mgb200_cugraph_params *pa
     if (e != cudaSuccess) return cuda_fail(e, "cudaMemcpyAsync(ranks D2H)", __FILE__, __LINE__);
   }
   if (stats_out) *stats_out = stats;
+  return MGB200_OK;
+}
+
+int mgb200_graph_gather(mgb200_graph *h, const double *x, double *y, int on_device, int weighted) {
+  if (!h) return MGB200_ERR_INVALID_ARGUMENT;
+  Graph &g = h->g;
+  if (g.part_world != 1) {
+    set_error("mgb200_graph_gather needs a single-partition graph");
+    return MGB200_ERR_INVALID_ARGUMENT;
+  }
+  if (g.n > 0 && (!x || !y)) {
+    set_error("x / y is null");
+    return MGB200_ERR_INVALID_ARGUMENT;
+  }
+  MGB_CUDA(cudaSetDevice(g.device));
+  if (g.n == 0) return MGB200_OK;
+  if (on_device) return gather_once(g, x, y, weighted != 0);
+  DeviceBuffers tmp;
+  double *d_x = nullptr, *d_y = nullptr;
+  MGB_CUDA(tmp.alloc(&d_x, g.n));
+  MGB_CUDA(tmp.alloc(&d_y, g.n));
+  MGB_CUDA(cudaMemcpyAsync(d_x, x, g.n * sizeof(double), cudaMemcpyHostToDevice, g.stream));
+  if (const int rc = gather_once(g, d_x, d_y, weighted != 0)) return rc;
+  MGB_CUDA(cudaMemcpyAsync(y, d_y, g.n * sizeof(double), cudaMemcpyDeviceToHost, g.stream));
+  MGB_CUDA(cudaStreamSynchronize(g.stream));
   return MGB200_OK;
 }
 

@@ -100,7 +100,48 @@ __global__ void __launch_bounds__(kThreads) ppr_write_kernel(uint64_t n, const u
   for (uint64_t v = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < n; v += stride) out[v] = pr[label_of[v]];
 }
 
+// one gather's input: x by original id into the label space; clears the flags that stop the gather kernels
+__global__ void __launch_bounds__(kThreads) gather_in_kernel(uint64_t n, const uint32_t *label_of, const double *x,
+                                                             double *contrib_pad, IterState *state) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t v = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < n; v += stride)
+    contrib_pad[label_of[v]] = x[v];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    contrib_pad[n] = 0.0;  // the slot SELL padding entries read
+    state->done = 0;
+    state->error = 0;
+  }
+}
+
+// one gather's output: y by original id from the heavy sums, the SELL sums, or 0 for rows without in-edges
+__global__ void __launch_bounds__(kThreads) gather_out_kernel(uint64_t n, uint64_t n_heavy, uint64_t n_sell,
+                                                              const double *heavy_sums, const double *sell_sums,
+                                                              const uint32_t *label_of, double *y) {
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+  for (uint64_t v = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < n; v += stride) {
+    const uint64_t r = label_of[v];
+    y[v] = r < n_heavy ? heavy_sums[r] : (r < n_heavy + n_sell ? sell_sums[r - n_heavy] : 0.0);
+  }
+}
+
 }  // namespace
+
+// y = A^T x (weighted: A holds the edge weights) with one gather phase and no epilogue; d_x and d_y are n doubles on the
+// device in original vertex order.  Overwrites contrib(0), so the next run starts from its own initialisation.
+int gather_once(Graph &g, const double *d_x, double *d_y, bool weighted) {
+  MGB_CUDA(cudaSetDevice(g.device));
+  const uint64_t n = g.n;
+  if (n == 0) return MGB200_OK;
+  cudaStream_t st = g.stream;
+  double *contrib = g.contrib(0);
+  gather_in_kernel<<<partial_blocks(n), kThreads, 0, st>>>(n, g.label_of, d_x, contrib, g.state);
+  if (const int rc = launch_gather_phase(g, contrib, nullptr, /*heavy_row_sums=*/true, weighted)) return rc;
+  gather_out_kernel<<<partial_blocks(n), kThreads, 0, st>>>(n, g.n_heavy, g.n_sell, g.heavy_sums, g.sell_sums, g.label_of,
+                                                            d_y);
+  MGB_CUDA(cudaGetLastError());
+  MGB_CUDA(cudaStreamSynchronize(st));
+  return MGB200_OK;
+}
 
 int cugraph_pagerank_iterate(Graph &g, const mgb200_cugraph_params &prm, double *d_out_original_order,
                              mgb200_cugraph_stats *stats) {

@@ -167,6 +167,18 @@ class PageRankGraph:
                                            ctypes.byref(st)))
         return out, _stats(st)
 
+    def gather(self, x, weighted=False):
+        """y = A^T x through the gather every algorithm on this layout iterates (mgb200_graph_gather): ``y[v]`` is the
+        sum of ``x[u]`` over the edges u -> v, each times its weight when ``weighted``.  ``x`` and the returned float64
+        array are in original vertex order.  Single-partition handles only."""
+        n = self.get_node_count()
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.shape != (n,):
+            raise MgB200Error(N.ERR_INVALID_ARGUMENT, f"x must hold {n} values")
+        y = np.empty(n, dtype=np.float64)
+        _check(N.lib().mgb200_graph_gather(self._h, x.ctypes.data if n else None, y.ctypes.data if n else None, 0,
+                                           1 if weighted else 0))
+        return y
 
     # ---- multi-GPU: one partition per GPU (mgb200_pagerank.h "multi-GPU" section) ----------------------
 
