@@ -233,6 +233,37 @@ int mgb200_bipartite_matching_run(mgb200_bfs_graph *g, int (*should_abort)(void 
 int mgb200_maximum_bipartite_matching(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to,
                                       uint64_t *matched_out);
 
+/*
+ * Strongly connected components on the same device graph: the partition of networkx.strongly_connected_components on
+ * the MultiDiGraph of all vertices and edges (the reference's nxalg.strongly_connected_components).  Self-loops and
+ * multi-edges change nothing.  component_out[v] is the number of v's component; components are numbered in the order
+ * of their smallest vertex id, as in mgb200_wcc_run, so the output is canonical.  Multistep: a trim of the vertices
+ * with no live in- or out-entry, a forward-backward search from a pivot, then colouring rounds; all integer work, so two
+ * runs give byte-identical outputs and stats (run_ms aside).  A vertex's entries count in 32 bits (degree < 2^32).
+ * Without a device every call fails with MGB200_ERR_CUDA.
+ */
+typedef struct mgb200_scc_stats {
+  uint64_t components;        /* number of components                                                              */
+  uint64_t largest_component; /* vertices in the largest one                                                       */
+  uint64_t trimmed;           /* singleton components removed by the trim                                          */
+  uint64_t pivot_component;   /* vertices of the component found by forward-backward from the pivot (0: none)      */
+  uint64_t coloring_rounds;   /* colour-then-collect rounds after forward-backward                                 */
+  uint64_t levels;            /* frontier levels of the forward, backward and propagation searches                 */
+  uint64_t host_round_trips;  /* device-to-host waits of the run (trim levels, pivot, searches and colouring)       */
+  uint64_t edges_inspected;   /* adjacency entries read: trim and searches together                                */
+  double run_ms;              /* CUDA-event time, first kernel .. last label written (no transfers)                */
+  uint64_t kernel_launches;
+} mgb200_scc_stats;
+
+/* component_out: n int64 values in host memory; stats may be NULL.  should_abort (may be NULL) is polled between host
+ * round trips; non-zero -> MGB200_ERR_ABORTED and component_out is left untouched.  n == 0 returns MGB200_OK with zero
+ * components and zero launches. */
+int mgb200_scc_run(mgb200_bfs_graph *g, int (*should_abort)(void *user), void *abort_user, int64_t *component_out,
+                   mgb200_scc_stats *stats);
+/* One shot on device 0: host COO (uint64 endpoints < n) -> component_out[n] in host memory. */
+int mgb200_strongly_connected_components(uint64_t n, uint64_t m, const uint64_t *from, const uint64_t *to,
+                                         int64_t *component_out);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -60,6 +60,12 @@ class MatchingStats(ctypes.Structure):
                 ("max_levels", u32), ("edges_inspected", u64), ("run_ms", f64), ("kernel_launches", u64)]
 
 
+class SccStats(ctypes.Structure):
+    _fields_ = [("components", u64), ("largest_component", u64), ("trimmed", u64), ("pivot_component", u64),
+                ("coloring_rounds", u64), ("levels", u64), ("host_round_trips", u64), ("edges_inspected", u64),
+                ("run_ms", f64), ("kernel_launches", u64)]
+
+
 class KatzStats(ctypes.Structure):
     _fields_ = [("iterations", u64), ("max_out_degree", u64), ("gamma", f64), ("iterate_ms", f64),
                 ("kernel_launches", u64), ("tie_order_runs", u64)]
@@ -134,6 +140,8 @@ EXPORTS = {
     "mgb200_weighted_shortest_paths": (i32, [u64, u64, vp, vp, vp, u64, i32, ctypes.c_int64, vp, vp]),
     "mgb200_bipartite_matching_run": (i32, [vp, ABORT_FN, vp, vp, vp, ctypes.POINTER(MatchingStats)]),
     "mgb200_maximum_bipartite_matching": (i32, [u64, u64, vp, vp, ctypes.POINTER(u64)]),
+    "mgb200_scc_run": (i32, [vp, ABORT_FN, vp, vp, ctypes.POINTER(SccStats)]),
+    "mgb200_strongly_connected_components": (i32, [u64, u64, vp, vp, vp]),
     # include/mgb200_katz.h
     "mgb200_katz_run": (i32, [vp, f64, f64, u64, vp, ctypes.POINTER(KatzStats)]),
     "mgb200_katz_centrality": (i32, [u64, u64, vp, vp, f64, f64, u64, vp, ctypes.POINTER(u64)]),

@@ -5,7 +5,8 @@
     memgraph_b200/_build/libmgp_fake_host.so     fake mgp host used by the tests to load query modules without Memgraph
     memgraph_b200/_build/<module>.so             the other query modules (gpu_bfs, katz_centrality, betweenness_centrality,
                                                  weakly_connected_components, bridges, biconnected_components,
-                                                 gpu_wsp, bipartite_matching, cugraph.* including cugraph.hits),
+                                                 gpu_wsp, bipartite_matching, strongly_connected_components,
+                                                 cugraph.* including cugraph.hits),
                                                  same linking as pagerank.so
 
 Objects are rebuilt only when a source or header is newer.  `python -m memgraph_b200.build` builds everything.
@@ -33,7 +34,7 @@ NVCC_FLAGS = [
     "-diag-suppress", "1444",  # cub::TransformInputIterator deprecation notice
 ]
 CUDA_SOURCES = ["pagerank_kernels.cu", "graph_build.cu", "capi.cu", "bfs.cu", "katz.cu", "personalized.cu", "betweenness.cu",
-                "wcc.cu", "biconnectivity.cu", "wsp.cu", "hits.cu", "bipartite_matching.cu"]
+                "wcc.cu", "biconnectivity.cu", "wsp.cu", "hits.cu", "bipartite_matching.cu", "scc.cu"]
 HEADERS = [os.path.join(CSRC, "core.hpp"), os.path.join(CSRC, "bfs_graph.hpp"), os.path.join(CSRC, "rmat.hpp"), os.path.join(CSRC, "sell_stream.cuh"),
            os.path.join(CSRC, "union_find.cuh"), os.path.join(CSRC, "undirected_walk.cuh"),
            os.path.join(INCLUDE, "mgb200_pagerank.h"), os.path.join(INCLUDE, "mgb200_bfs.h"),
@@ -95,6 +96,8 @@ MODULES = {
                                    ("biconnected_components.so", ["-DMGB200_BRIDGES=0"], "biconnected_components_module")],
     "gpu_wsp_module.cpp": [("gpu_wsp.so", [], "wsp_module")],
     "bipartite_matching_module.cpp": [("bipartite_matching.so", [], "bipartite_matching_module")],
+    "strongly_connected_components_module.cpp": [("strongly_connected_components.so", [],
+                                                  "strongly_connected_components_module")],
 }
 
 # The fake mgp hosts the tests load modules through (test infrastructure, so they live with the tests): library ->

@@ -1,6 +1,7 @@
 """Connectivity on the device (include/mgb200_bfs.h): the host-side mirrors of the reference's
 ``weakly_connected_components.get`` (mage/cpp/connectivity_module/connectivity_module.cpp:41-84), ``bridges.get`` and
-``biconnected_components.get`` (mage/cpp/bridges_module, mage/cpp/biconnected_components_module).  They run on a
+``biconnected_components.get`` (mage/cpp/bridges_module, mage/cpp/biconnected_components_module), and the strongly
+connected components of ``nxalg.strongly_connected_components`` (query_modules/nxalg.py).  They run on a
 :class:`memgraph_b200.bfs.BfsGraph` handle -- the same device-resident CSR + CSC as BFS and betweenness."""
 import ctypes
 
@@ -27,6 +28,27 @@ def weakly_connected_components(n, sources, targets):
     out = np.zeros(int(n), dtype=np.int64)
     _check(N.lib().mgb200_weakly_connected_components(int(n), len(s), s.ctypes.data, t.ctypes.data,
                                                       out.ctypes.data if n else None))
+    return out
+
+
+def scc_run(graph, should_abort=None):
+    """Strongly connected component of every vertex, numbered in the order of each component's smallest vertex id.
+    ``should_abort`` (a callable returning true to stop) is polled between host round trips; a stop raises
+    MgB200Error with code ERR_ABORTED.  -> (int64[n], stats dict)."""
+    out = np.zeros(graph.n, dtype=np.int64)
+    st = N.SccStats()
+    cb = N.ABORT_FN(lambda _user: 1 if should_abort() else 0) if should_abort else N.ABORT_FN()
+    _check(N.lib().mgb200_scc_run(graph._h, cb, None, out.ctypes.data if graph.n else None, ctypes.byref(st)))
+    return out, {k: getattr(st, k) for k, _ in N.SccStats._fields_}
+
+
+def strongly_connected_components(n, sources, targets):
+    """One shot on device 0: int64[n] strongly connected component of every vertex, numbered in the order of each
+    component's smallest vertex id."""
+    s, t = _coo(sources, targets)
+    out = np.zeros(int(n), dtype=np.int64)
+    _check(N.lib().mgb200_strongly_connected_components(int(n), len(s), s.ctypes.data, t.ctypes.data,
+                                                        out.ctypes.data if n else None))
     return out
 
 
@@ -67,4 +89,4 @@ def biconnected_components(n, sources, targets):
 
 
 __all__ = ["BfsGraph", "wcc_run", "weakly_connected_components", "biconnectivity_run", "bridges",
-           "biconnected_components"]
+           "biconnected_components", "scc_run", "strongly_connected_components"]

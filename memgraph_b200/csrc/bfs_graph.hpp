@@ -1,7 +1,8 @@
 // memgraph_b200/csrc/bfs_graph.hpp -- the device graph behind the opaque mgb200_bfs_graph handle (include/mgb200_bfs.h).
 // Shared by the breadth-first expansion (bfs.cu), which builds it, betweenness centrality (betweenness.cu), weakly
-// connected components (wcc.cu), bridges and biconnected components (biconnectivity.cu) and weighted shortest paths
-// (wsp.cu), which walk the same CSR + CSC; also the grid-stride and warp helpers of their kernels.
+// connected components (wcc.cu), bridges and biconnected components (biconnectivity.cu), weighted shortest paths
+// (wsp.cu), bipartite matching (bipartite_matching.cu) and strongly connected components (scc.cu), which walk the same
+// CSR + CSC; also the grid-stride and warp helpers of their kernels.
 #pragma once
 
 #include <cuda_runtime.h>

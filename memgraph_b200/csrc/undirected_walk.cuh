@@ -1,6 +1,7 @@
 // memgraph_b200/csrc/undirected_walk.cuh -- the entry walk over the undirected view of the BFS device graph and the
 // breadth-first spanning forest built with it, shared by bridges / biconnected components (biconnectivity.cu) and
-// maximum bipartite matching (bipartite_matching.cu).
+// maximum bipartite matching (bipartite_matching.cu).  Strongly connected components (scc.cu) walk directed lists with
+// the same walk(): its scheduler only asks op.g.degree(u), so an op whose g is one direction's lists walks those.
 //
 // walk      an op visits the entries [rank, degree) of a vertex with stride `width`: a thread per vertex up to
 //           kThreadEntries entries, a warp up to kWarpEntries and a block above, so hubs do not serialise a pass

@@ -14,15 +14,14 @@
 //   finish    every unmarked vertex links with the remaining entries of its undirected list, from position
 //             kSampleRounds on.  An edge u -> w whose u is marked is still seen from w's in-list, so skipping the
 //             giant's members loses no edge; then one more compression
-//   label     flag = (parent[v] == v), exclusive scan of the flags, component[v] = scan[parent[v]]
+//   label     flag = (parent[v] == v), exclusive scan of the flags, component[v] = scan[parent[v]] (number_sets,
+//             union_find.cuh)
 // The link hooks the larger of two roots under the smaller one with atomicCAS, and a compression only shortens paths,
 // so parent[x] <= x always holds and every root is its component's smallest id, whatever order the threads link in.
 // The output is integers: two runs are byte-identical.  The finish runs a thread per vertex up to kThreadEntries
 // remaining entries, a warp per vertex up to kWarpEntries and a block per vertex above that (RMAT in-degrees reach
 // about 10^6 at scale 26).
 #include <cub/cub.cuh>
-#include <thrust/iterator/counting_iterator.h>
-#include <thrust/iterator/transform_iterator.h>
 
 #include <algorithm>
 #include <cstdint>
@@ -185,16 +184,6 @@ __global__ void __launch_bounds__(kThreads) size_kernel(uint64_t n, const uint32
   if (threadIdx.x == 0 && block_giant) atomicAdd(size + giant, block_giant);
 }
 
-struct IsRoot {
-  const uint32_t *parent;
-  __device__ __forceinline__ uint32_t operator()(uint64_t v) const { return parent[v] == v ? 1u : 0u; }
-};
-
-__global__ void __launch_bounds__(kThreads) label_kernel(uint64_t n, const uint32_t *parent, const uint32_t *scan,
-                                                         int64_t *component) {
-  for (uint64_t v = first_thread(); v < n; v += thread_count()) component[v] = scan[parent[v]];
-}
-
 // The most frequent value; ties go to the smaller one.
 uint32_t most_frequent(std::vector<uint32_t> values) {
   std::sort(values.begin(), values.end());
@@ -248,9 +237,8 @@ int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats
   MGB_CUDA(buf.alloc(&largest, 1));
   MGB_CUDA(buf.alloc(&component, n));
   MGB_CUDA(buf.alloc(&counters, 1));
-  const auto flags = thrust::make_transform_iterator(thrust::counting_iterator<uint64_t>(0), IsRoot{parent});
   size_t scan_bytes = 0, max_bytes = 0;
-  MGB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, flags, scan, n, st));
+  MGB_CUDA(number_sets(n, parent, scan, component, nullptr, &scan_bytes, 1, st));
   MGB_CUDA(cub::DeviceReduce::Max(nullptr, max_bytes, size, largest, n, st));
   char *cub_tmp = nullptr;
   MGB_CUDA(buf.alloc(&cub_tmp, std::max(scan_bytes, max_bytes)));
@@ -287,8 +275,7 @@ int mgb200_wcc_run(mgb200_bfs_graph *g, int64_t *component_out, mgb200_wcc_stats
   size_kernel<<<grid, kThreads, 0, st>>>(n, parent, giant_root, size);
   stats.kernel_launches++;
   MGB_CUDA(cub::DeviceReduce::Max(cub_tmp, max_bytes, size, largest, n, st));
-  MGB_CUDA(cub::DeviceScan::ExclusiveSum(cub_tmp, scan_bytes, flags, scan, n, st));
-  label_kernel<<<grid, kThreads, 0, st>>>(n, parent, scan, component);
+  MGB_CUDA(number_sets(n, parent, scan, component, cub_tmp, &scan_bytes, grid, st));  // scan + label_kernel
   stats.kernel_launches++;
   MGB_CUDA(cudaGetLastError());
   MGB_CUDA(cudaEventRecord(g->ev1, st));
